@@ -1,7 +1,7 @@
-"""In-tree build of libaerial_gym_b200.so (nvcc, sm_100a only).
+"""In-tree build of libaerial_gym_b200.so (nvcc, sm_90a only: H100).
 
 ``python -m aerial_gym_simulator_b200._build`` or ``__graft_entry__.build()``.
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot."""
+The .so and the objects under build/ are git-ignored build products."""
 import os
 import subprocess
 import sys
@@ -13,10 +13,9 @@ LIB = os.path.join(PKG, "libaerial_gym_b200.so")
 # fmaf() so that the C oracle (oracle/hp2_oracle.c, -ffp-contract=off) is bit-reproducible.
 UNITS = [
     ("agx_common.cu", []),
-    # hp1: 2-ulp division / sqrt (no slow-path branches): the step is instruction-fetch bound at
-    # 65,536 envs (profiles/hp1_step_r1.md: stall_no_instruction dominates), every instruction counts
-    # AGX_HP1_NOINLINE_TRIG: one shared out-of-line sincosf instead of seven inlined copies (same function, same bits): -2..5 % step time
-    ("hp1.cu", ["-prec-div=false", "-prec-sqrt=false", "-DAGX_HP1_NOINLINE_TRIG"]),  # AGX_FAST_TRIG measured: -7% time, 3x parity error -> off
+    # hp1: 2-ulp division / sqrt (no slow-path branches): the step is a long dependent chain per warp, every instruction counts
+    # AGX_HP1_NOINLINE_TRIG: one shared out-of-line sincosf instead of seven inlined copies (same function, same bits)
+    ("hp1.cu", ["-prec-div=false", "-prec-sqrt=false", "-DAGX_HP1_NOINLINE_TRIG"]),  # AGX_FAST_TRIG: 3x parity error -> off
     ("hp1_aux.cu", []),
     ("lidar_nav.cu", []),
     # device-RNG units: no FMA contraction, so "lo + (hi - lo) u" and the noise model round like their numpy oracles
@@ -29,7 +28,7 @@ UNITS = [
     ("p2p_allgather.cu", []),
 ]
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
 ]
 
@@ -39,6 +38,12 @@ def _nvcc():
         if c and (os.path.isabs(c) and os.path.exists(c) or not os.path.isabs(c)):
             return c
     raise RuntimeError("nvcc not found")
+
+
+def cuda_tool(name):
+    """a CUDA toolkit binary (cuobjdump, ...) from the same toolkit as nvcc"""
+    nvcc = _nvcc()
+    return os.path.join(os.path.dirname(nvcc), name) if os.path.isabs(nvcc) else name
 
 
 def sources():
@@ -71,7 +76,7 @@ def build(force=False, verbose=False):
         if r.returncode:
             raise RuntimeError(f"nvcc failed for {unit}")
         objs.append(obj)
-    cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB] + objs
+    cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", LIB] + objs
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode:
         sys.stderr.write(r.stdout + r.stderr)

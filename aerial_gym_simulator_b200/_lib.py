@@ -153,7 +153,7 @@ def load():
     if not os.path.exists(path):
         raise AgxError(
             f"{path} not found: build it with `python -m aerial_gym_simulator_b200._build` "
-            "(nvcc, sm_100a).  There is no CPU / torch fallback."
+            "(nvcc, sm_90a).  There is no CPU / torch fallback."
         )
     lib = C.CDLL(path)
     lib.agx_abi_version.restype = C.c_int

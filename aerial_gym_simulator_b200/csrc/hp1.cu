@@ -1,4 +1,4 @@
-// HP1: fused multirotor step for sm_100a.
+// HP1: fused multirotor step for sm_90a (H100).
 //
 //   update_states -> Lee controller -> allocation -> motor model -> drag/disturbance ->
 //   rigid-body integrate  (x physics_steps)  [-> position-task reward / flags / reset / obs]
@@ -271,8 +271,8 @@ AGX_HP1_RESET_FN void reset_one_env(const AgxHp1Config& cfg, const AgxHp1Buffers
 // (3) Multi-GPU: the step kernel never touches NVLink and never waits for the gather.  With an observation all-gather attached
 // (agx_obs_gather_push, p2p_allgather.cu, on side streams) buf.obs is one slot of a ring the push kernels read asynchronously; the
 // HOST keeps a step from overwriting a slot whose push has not finished (stream events) -- an in-kernel wait here would let the
-// blocked step's CTAs and their chained successors hold every CTA slot the pending push needs (measured: round 2, 2 GPUs, deadlock
-// until the wall-clock bound fired, profiles/p2p_2gpu_r2c_ring_backpressure_deadlock.log).
+// blocked step's CTAs and their chained successors hold every CTA slot the pending push needs (a deadlock until the wall-clock
+// bound fires: tests/test_gather_protocol_model.py).
 #ifdef AGX_TIMELINE  // debug builds only (tools/dbg/timeline.py): per-warp start / end globaltimer stamps
 __device__ unsigned long long g_timeline[4][8192];
 __device__ __forceinline__ unsigned long long gtimer() {
@@ -307,9 +307,8 @@ hp1_step_kernel(const __grid_constant__ AgxHp1Config cfg, const __grid_constant_
     if constexpr (COOP) {
         const int my_tile = blockIdx.x * kWarpsPerBlock + warp;
         const bool has_tile = my_tile < n_tiles;
-        // (Round 2 tried fetching the tile's done-counter and the four arrival counters together with the claim -- one round trip
-        // instead of three.  Measured (profiles/hp1_bisect_r2i.jsonl): 2048 extra loads per step on the line the arrival atomics
-        // hammer made the dependent-chain loop 4 us SLOWER; the acquire spins below touch that line only when they must.)
+        // (The tile's done-counter and the four arrival counters are NOT fetched together with the claim: extra loads on the line the
+        // arrival atomics hammer slow the dependent-chain loop; the acquire spins below touch that line only when they must.)
         if (has_tile && lane == 0) step_T = atomicAdd(buf.tile_sync + my_tile, 1u);  // claim: which step of this tile am I?
         step_T = __shfl_sync(0xffffffffu, step_T, 0);
         __syncthreads();  // every warp of the CTA holds its claim before the CTA lets the next launch in
@@ -449,7 +448,9 @@ AGX_HP1_MOTOR_UNROLL
         AGX_TL(1);
         bool do_reset = false;
         int flag_pre = 0;
-        if constexpr (COOP) flag_pre = (*reinterpret_cast<volatile uint32_t*>(reset_flag) == flag_tag);  // consumed after the epilogue
+        // warp-uniform (consumed after the epilogue): in a partial tile the lanes may arrive here diverged, at different times; a flag
+        // raised in between would give lanes of one warp different decisions below and a full-mask __any_sync only some of them reach
+        if constexpr (COOP) flag_pre = __any_sync(0xffffffffu, *reinterpret_cast<volatile uint32_t*>(reset_flag) == flag_tag);
         if constexpr (TASK) {
             int steps = steps_in + 1;  // env_manager.py:429
             if (valid) {
@@ -523,7 +524,7 @@ AGX_HP1_MOTOR_UNROLL
                     const unsigned long long* cnt = arrive_ctr;
                     // until the flag rises, or every warp of this step has arrived (then the flag is final)
                     spin_until([&] { return *fl == flag_tag || ld_acquire_gpu_u64(cnt) >= arrive_target; }, buf.any_reset, 3 | (int)(step_T << 4));
-                    any = (*fl == flag_tag);
+                    any = __any_sync(0xffffffffu, *fl == flag_tag);  // the flag is monotonic: one lane seeing it raised means it is
                 }
                 // ---- derived states for the observation: one common pass for resetting envs (new state)
                 // and, if anybody reset, for everybody else (post-physics state) ------------------------
@@ -764,9 +765,14 @@ inline int coop_capacity(StepKernel k) {
     return cap;
 }
 // CTA slots kept free for kernels that run BESIDE the chained step (the observation gather's push kernel): the one-sided grid
-// barrier needs every CTA of a step resident, so the step only takes the single-launch path when it fits with this margin
+// barrier needs every CTA of a step resident, so the step only takes the single-launch path when it fits with this margin.
+// What liveness needs is one slot per ring slot, for the one-warp ready gates (tests/_protocol_model.py): a push CTA only becomes
+// resident after its ready gate has seen the step published, so the push CTAs themselves (256 threads each: 24 of them take the
+// threads of 96 step CTAs) need not fit beside the step.  32 is that bound for a ring of 4 plus margin; the margin is not measured on
+// multi-GPU H100s.  H100: 132 SMs x 8 = 1056 slots - 32 = 1024 = exactly the grid of 65,536 envs.  Any loss of occupancy or fewer
+// SMs moves that size to the two-launch path (same results, slower): bench.py's config5_env_sweep reports the path per size.
 #ifndef AGX_HP1_COOP_RESERVE
-#define AGX_HP1_COOP_RESERVE (192 / AGX_HP1_WARPS_PER_BLOCK)  // 96 two-warp CTAs = 96 x 8192 registers
+#define AGX_HP1_COOP_RESERVE 32
 #endif
 constexpr int kCoopReserve = AGX_HP1_COOP_RESERVE;
 inline int grid_for(int n_envs) {

@@ -1,4 +1,4 @@
-// HP2: depth / segmentation / LiDAR ray-caster for sm_100a.
+// HP2: depth / segmentation / LiDAR ray-caster for sm_90a (H100).
 //
 //   agx_hp2_update_scene : per env (one CTA): instance transform of template triangles into
 //                          world space, object AABBs, 30-bit Morton codes, bitonic sort in shared
@@ -1053,7 +1053,7 @@ int agx_hp2_cast(const AgxHp2Scene* sc, const AgxHp2Sensor* sn, void* stream) {
     if ((sn->kind == AGX_SENSOR_LIDAR || sn->kind == AGX_SENSOR_NORMAL_FACEID_LIDAR) && !sn->ray_table)
         return agx_set_error(AGX_E_NULL, "LiDAR needs ray_table");
     if (sn->robot_pose_stride < 7) return agx_set_error(AGX_E_INVALID, "robot_pose_stride < 7");
-    int dev = 0, sms = 148, max_smem = 0;
+    int dev = 0, sms = 132, max_smem = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     cudaDeviceGetAttribute(&max_smem, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);

@@ -1,7 +1,6 @@
-// Observation all-gather as a single kernel of NVLink peer stores + flag handshake (B200 / NVSwitch:
+// Observation all-gather as a single kernel of NVLink peer stores + flag handshake (H100 / NVSwitch:
 // every peer is reachable at full bandwidth, so each rank simply writes its shard into every
-// peer's buffer).  Used instead of an NCCL collective on the step path: at 65,536 envs a step is
-// ~20 us, shorter than an NCCL launch.
+// peer's buffer).  Used instead of an NCCL collective on the step path, where a step is too short to hide an NCCL launch.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -316,7 +315,7 @@ extern "C" int agx_p2p_allgather(const void* local, void* const* peer_bufs, uint
     if (bytes % 16 || ((uintptr_t)local & 15)) return agx_set_error(AGX_E_INVALID, "p2p_allgather: bytes and local must be 16-byte aligned");
     if (bytes == 0) return AGX_OK;
     size_t n_vec = bytes / 16;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     long long blocks = (long long)((n_vec + 255) / 256);

@@ -29,7 +29,11 @@ extern "C" int agx_hp2_noise_limits(float* pixels, uint64_t num_pixels, uint64_t
     if (num_pixels == 0) return AGX_OK;
     if (!pixels) return agx_set_error(AGX_E_NULL, "agx_hp2_noise_limits: pixels is NULL");
     const uint64_t want = (num_pixels + kNoiseThreads - 1) / kNoiseThreads;
-    const int blocks = (int)(want < (uint64_t)(148 * 32) ? want : (uint64_t)(148 * 32));  // <= 32 CTAs per SM worth of grid-stride work
+    int dev = 0, sms = 132;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const uint64_t cap = (uint64_t)sms * 32;  // <= 32 CTAs per SM worth of grid-stride work
+    const int blocks = (int)(want < cap ? want : cap);
     noise_limits_kernel<<<blocks, kNoiseThreads, 0, (cudaStream_t)stream>>>(pixels, num_pixels, first_pixel, *cfg, frame, (uint32_t)(seed & 0xffffffffu),
                                                                            (uint32_t)(seed >> 32));
     return agx_check_launch("noise_limits_kernel");

@@ -170,7 +170,7 @@ class PipelinedObsGather:
         self.local_count, self.feat = local_count, feat
         i64 = lambda ptrs: torch.tensor(list(ptrs), dtype=torch.int64, device=self.device)
         self._handles, self.mc_ptrs = [], []
-        if multicast is None:  # measured (profiles/gather_bench_*gpu_r2*.log): 2 GPUs 14.9 vs 13.8 us/step (slower), 4 GPUs 22.3 vs 25.5, 8 GPUs 39.9 vs 49.1
+        if multicast is None:
             env = os.environ.get("AGX_GATHER_MULTICAST")
             multicast = (env != "0") if env is not None else None
         B = self.num_buffers

@@ -1,5 +1,5 @@
 """EnvManager: the orchestrator surface of the reference (env_manager/env_manager.py) over the
-B200 engines.  Registers the env / sim configs (env_manager/__init__.py, sim/__init__.py)."""
+H100 engines.  Registers the env / sim configs (env_manager/__init__.py, sim/__init__.py)."""
 from ..config import env_config as _ec
 from ..config import sim_config as _sc
 from ..registry._core import env_config_registry, sim_config_registry

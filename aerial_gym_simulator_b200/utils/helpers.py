@@ -27,7 +27,7 @@ def class_to_dict(obj) -> dict:
     return out
 
 
-def parse_arguments(description="B200 aerial gym", headless=False, no_graphics=False, custom_parameters=[]):
+def parse_arguments(description="H100 aerial gym", headless=False, no_graphics=False, custom_parameters=[]):
     p = argparse.ArgumentParser(description=description)
     if headless:
         p.add_argument("--headless", action="store_true")

@@ -12,12 +12,12 @@ observation and (N > 1) the all-gather of the observation tensor: hand-written N
 kernels that run BESIDE the chained step launches on a side stream (the push of step t overlaps step
 t+1; the K-th gather has landed on every rank before the closing event; --gather sync|nccl for the
 per-step-awaited and the NCCL variants).  The step of an 8-GPU run must RECEIVE 7 x 3.4 MB of rows:
-`roofline.nvlink_floor_us` = that ingress / 900 GB/s is the floor of the step period at N > 1.
+`roofline.nvlink_floor_us` = that ingress / 450 GB/s (H100 NVLink, one direction) is the floor of the step period at N > 1.
 
 Timing: W >= 3 warm-up steps, then exactly K steps bracketed by barrier + synchronize and one
-CUDA-event pair on the launching stream.  One 65,536-env working set (~12 MB) is smaller than the
-126 MB L2, so the timed loop rotates over R = 16 independent replicas of the environment batch
-(~190 MB of state in total, larger than L2): every step finds its state cold in L2, nothing is
+CUDA-event pair on the launching stream.  One 65,536-env working set (~12 MB) fits in the H100's
+50 MB L2, so the timed loop rotates over R = 16 independent replicas of the environment batch
+(~190 MB of state in total, several times L2): every step finds its state cold in L2, nothing is
 flushed and no step is skipped.  value = N_gpus * envs * K / elapsed, max over ranks.
 `value_hot_l2` is the same loop on a single replica (state resident in L2; every tile's step waits for
 that tile's previous step -- the dependent-chain figure, what a policy-free rollout of ONE batch sees).
@@ -329,6 +329,8 @@ def run_ours(args):
         dist.all_reduce(total_ms, op=dist.ReduceOp.MAX)
     total_s = float(total_ms.item()) * 1e-3
     value = world * N * K / total_s
+    if args.dump_outputs and rank == 0:  # before the loops below step the same engines again
+        dump_outputs(args.dump_outputs, last["engine"])
 
     # ---- N > 1: (a) self-check -- the gathered buffer of the last timed step equals the library collective's gather of the same
     # observation, on every rank; (b) the same loop with the gather awaited after EVERY step (what a policy in the loop sees) ----
@@ -525,19 +527,14 @@ def run_ours(args):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)" if "hbm_gbs" in peaks else "fallback 6.65 TB/s"
+        peak = float(peaks.get("hbm_gbs", 3350.0))
+        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)" if "hbm_gbs" in peaks else "fallback 3.35 TB/s (H100 SXM data sheet)"
         # the timed region is K back-to-back launches of the one step kernel bracketed by one CUDA-event pair:
         # average launch duration = region / K.  (A per-launch event pair serialises the launches -- no
         # programmatic-dependent-launch overlap -- and adds the event's own latency: reported separately.)
         main_iso_s = float(main_total.item()) * 1e-3 / Kk
         main_avg_s = total_s / K
         achieved = ALG_BYTES_PER_ENV_STEP * N / main_avg_s / 1e9
-        traffic = None
-        try:
-            traffic = json.load(open(os.path.join(ROOT, "profiles", "hp1_traffic.json"))).get("dram_bytes_per_launch")
-        except Exception:
-            pass
         cpu = None
         if world == 1 and not args.no_cpu_baseline:
             v, per, cores, kind, note = time_cpu_reference(ENVS_PER_GPU, 40, 3)
@@ -557,14 +554,14 @@ def run_ours(args):
             "wall_s_timed_region": t_wall,
             "host_enqueue_us_per_step": 1e6 * t_enqueue / K,
             "roofline": {"bound": "hbm", "kernel": "hp1_step_kernel<4,true,true> (the whole fused step is this one launch)", "achieved": achieved, "peak": peak,
-                         "unit": "GB/s", "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
+                         "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src,
                          "algorithmic_bytes_per_launch": ALG_BYTES_PER_ENV_STEP * N,
-                         "nvlink_floor_us": ((world - 1) * N * 13 * 4 / 900e9 * 1e6) if world > 1 else None,
+                         "nvlink_floor_us": ((world - 1) * N * 13 * 4 / 450e9 * 1e6) if world > 1 else None,
                          "kernel_ms_avg": main_avg_s * 1e3,
                          "kernel_ms_isolated_event_pair": main_iso_s * 1e3,
                          "note": "at 65,536 envs the launch is ~14 MB: FP32 dependent-chain latency bound, not HBM bound (DESIGN.md). "
-                                 "kernel_ms_avg = timed region / K launches; launches are chained per tile and overlap in flight, one "
-                                 "launch alone spans ~11.5 us (tools/dbg/timeline.py) and 17-19 us when serialised by its own event pair / ncu"},
+                                 "kernel_ms_avg = timed region / K launches; launches are chained per tile and overlap in flight, so one "
+                                 "launch serialised by its own event pair (kernel_ms_isolated_event_pair) takes longer"},
             "cpu_baseline": cpu,
             "e2e": {"value": e2e_value, "unit": "env-steps/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                     "value_memcpy_variant": e2e_memcpy, "sharded_task_obs_equals_nccl": e2e_gather_ok,
@@ -588,6 +585,29 @@ def run_ours(args):
     if world > 1:
         dist.destroy_process_group()
     return 0
+
+
+DUMP_MAX_BYTES = 64_000_000  # 64 MB in all, in decimal units (also under 64 MiB)
+
+
+def dump_outputs(out_dir, e):
+    """DIR/<name>.npy (float32; env_index float64) of what the last timed step handed its caller: observation, reward, termination and truncation flags
+    and the root state.  Past DUMP_MAX_BYTES in all (.npy headers included) the same fixed, seeded sample of env rows is kept from every
+    array, and its row indices are written as env_index.npy.  At N > 1 this is rank 0's shard (its rows of the gathered observation)."""
+    import numpy as np
+
+    arrays = {"obs": e.obs, "reward": e.reward, "terminations": e.terminations, "truncations": e.truncations, "root_state": e.root_state}
+    arrays = {k: v.detach().cpu().float().numpy() for k, v in arrays.items()}
+    n = len(arrays["reward"])
+    row_bytes = sum(a[0].nbytes if a.ndim > 1 else a.itemsize for a in arrays.values())
+    budget = DUMP_MAX_BYTES - (64 << 10)  # room for the six .npy headers
+    if n * row_bytes > budget:
+        rows = np.sort(np.random.default_rng(0).choice(n, budget // (row_bytes + 8), replace=False))  # + 8: env_index is float64
+        arrays = {k: a[rows] for k, a in arrays.items()}
+        arrays["env_index"] = rows.astype(np.float64)
+    os.makedirs(out_dir, exist_ok=True)
+    for k, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{k}.npy"), np.ascontiguousarray(a))
 
 
 class _CamCfg:
@@ -615,7 +635,7 @@ def _peak_hbm():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return float(peaks["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
     except Exception:
-        return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+        return 3350.0, "fallback 3.35 TB/s (H100 SXM data sheet)"
 
 
 def cpu_ray_baseline(sensor, scene_np, robot_np, sample_envs):
@@ -832,7 +852,7 @@ def run_hp1_sweep(dev, world, rank, args, sizes):
         out.append({"envs_per_gpu": N, "global_envs": N * world, "value": val, "unit": "env-steps/s", "us_per_step": sec * 1e6 / K, "steps": K,
                     "replicas": R, "path": "single launch, chained per tile" if chained else "two launches (grid larger than one resident wave)",
                     "roofline_frac": ALG_BYTES_PER_ENV_STEP * N * K / sec / 1e9 / peak,
-                    "nvlink_floor_us": ((world - 1) * N * 52 / 900e9 * 1e6) if world > 1 else None})
+                    "nvlink_floor_us": ((world - 1) * N * 52 / 450e9 * 1e6) if world > 1 else None})
         for e in engines:
             if gather is not None:
                 e.attach_obs_gather(None)
@@ -913,6 +933,10 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--envs", type=int, default=ENVS_PER_GPU, help="envs per GPU (default: BASELINE configs[1])")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="write the observation, reward, flags and root state of the last timed step as DIR/<name>.npy (float32, at most "
+                         "64 MB: a fixed, seeded sample of env rows beyond that; at N > 1 rank 0's shard); inputs are seeded, so runs with the "
+                         "same arguments compare output for output")
     ap.add_argument("--gather", default="pipelined", choices=["pipelined", "sync", "nccl"],
                     help="N>1 observation all-gather: hand-written NVLink push / wait kernels beside the chained steps, the push of "
                          "step t overlapping step t+1 (default; actions are pre-generated, as at N=1); the same kernels awaited "

@@ -1,5 +1,5 @@
 /*
- * aerial_gym_b200 -- C ABI of the B200-native hot paths (libaerial_gym_b200.so).
+ * aerial_gym_b200 -- C ABI of the H100-native hot paths (libaerial_gym_b200.so).
  *
  * The reference (ntnu-arl/aerial_gym_simulator, commit f0d0f05) has NO plugin / FFI boundary
  * for these paths: they sit behind plain Python objects (SURVEY.md section 8b).  The entry

@@ -5,7 +5,7 @@ this module; only ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s
 ``cpu_baseline`` / ``--impl reference`` legs do, and only as the checker or the
 reported CPU baseline -- never as the product path.
 
-What it restates (reference = /root/reference/aerial_gym, commit f0d0f05):
+What it restates (reference = $AERIAL_GYM_REFERENCE/aerial_gym, commit f0d0f05):
 
 * quaternion helpers                      utils/math.py:58-65, 123-180, 242-293, 313-347
 * BaseMultirotor.update_states            robots/base_multirotor.py:287-294

@@ -4,7 +4,7 @@
  * TEST INFRASTRUCTURE ONLY: imported by tests/, __graft_entry__.smoke() and bench.py's
  * cpu_baseline / --impl reference legs, never by the product.
  *
- * What it restates (reference = /root/reference/aerial_gym, commit f0d0f05):
+ * What it restates (reference = $AERIAL_GYM_REFERENCE/aerial_gym, commit f0d0f05):
  *   - sensor pose compose                  sensors/warp/warp_sensor.py:177-187
  *   - camera ray generation + outputs      sensors/warp/warp_kernels/warp_camera_kernels.py:13-66,125-282
  *   - LiDAR ray generation + outputs       sensors/warp/warp_kernels/warp_lidar_kernels.py:13-163

@@ -29,7 +29,7 @@ import sys
 import tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_SRC = "/root/reference"
+from tests.golden._ref_loader import REF_ROOT as REF_SRC  # noqa: E402  (AERIAL_GYM_REFERENCE: a checkout of the reference)
 REF_DST = os.path.join(ROOT, "baseline", "_ref")
 
 
@@ -38,14 +38,14 @@ def staged() -> bool:
 
 
 def stage(force=False) -> str:
-    """Install the unmodified reference into baseline/_ref (git-ignored, travels to the GPU box).  Needs /root/reference."""
+    """Install the unmodified reference into baseline/_ref (git-ignored, travels to the GPU box).  Needs a reference checkout (AERIAL_GYM_REFERENCE)."""
     if staged() and not force:
         return REF_DST
     if not os.path.isdir(os.path.join(REF_SRC, "aerial_gym")):
-        raise RuntimeError("/root/reference is not present: the reference arm can only be staged in the build container")
+        raise RuntimeError("AERIAL_GYM_REFERENCE does not name a checkout of the reference: the reference arm cannot be staged")
     shutil.rmtree(REF_DST, ignore_errors=True)
     os.makedirs(REF_DST, exist_ok=True)
-    with tempfile.TemporaryDirectory() as tmp:  # /root/reference is read-only and the build writes into the source tree
+    with tempfile.TemporaryDirectory() as tmp:  # the reference checkout may be read-only and the build writes into the source tree
         src = os.path.join(tmp, "ref")
         shutil.copytree(REF_SRC, src, ignore=shutil.ignore_patterns(".git", "resources", "docs", "*.pth", "*.pt", "*.zip", "*.gif", "*.png"))
         r = subprocess.run([sys.executable, "-m", "pip", "install", "--no-index", "--no-build-isolation", "--no-deps", "--find-links",

@@ -1,9 +1,10 @@
-"""Import the *reference's own* torch control stack on CPU (this container only).
+"""Import the *reference's own* torch control stack on CPU.
 
-Test infrastructure, never imported by the product.  ``/root/reference`` does
-not travel to the GPU box, so this module is only used by
-``tests/golden/make_golden.py`` to produce the committed fixtures and by the
-optional ``-m "not gpu"`` cross-checks that skip when the reference is absent.
+Test infrastructure, never imported by the product.  The reference is a checkout of
+ntnu-arl/aerial_gym_simulator (commit f0d0f05) named by the ``AERIAL_GYM_REFERENCE``
+environment variable; it is not part of this repository.  This module is used by
+``tests/golden/make_golden*.py`` to produce the committed fixtures and by the
+optional ``-m "not gpu"`` cross-checks that skip when no reference is given.
 
 Procedure (SURVEY.md section 8c): register ``aerial_gym`` as a namespace module
 whose ``__path__`` points into the reference tree (this skips the package
@@ -17,7 +18,7 @@ import types
 
 import torch
 
-REF_ROOT = "/root/reference"
+REF_ROOT = os.environ.get("AERIAL_GYM_REFERENCE", "")
 
 
 def reference_available() -> bool:

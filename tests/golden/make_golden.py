@@ -2,10 +2,10 @@
 
     python tests/golden/make_golden.py
 
-Imports the reference control stack from /root/reference on CPU (see _ref_loader.py),
+Imports the reference control stack from $AERIAL_GYM_REFERENCE on CPU (see _ref_loader.py),
 drives ``BaseMultirotor.step`` / ``reset_idx`` / the position-task ``compute_reward`` with
 seeded inputs and stores inputs + outputs as small ``.npz`` fixtures next to this file.
-The fixtures travel to the GPU box; /root/reference does not.
+The fixtures travel to the GPU box; $AERIAL_GYM_REFERENCE does not.
 
 What is pinned: rows a1-a12, a15, a16 of SURVEY.md section 8.  What cannot be: the PhysX
 integrator (a13) and Warp traversal (b9) -- not in the tree, not installable.

@@ -3,7 +3,7 @@
     python tests/golden/make_golden_hp2.py
 
 The reference's `WarpSensor` (sensors/warp/warp_sensor.py) with its `WarpCam` / `WarpLidar` / `WarpStereoCam` / `WarpNormalFaceID*`
-classes and every `@wp.kernel` they launch are imported UNMODIFIED from /root/reference; `warp` itself (warp-lang 1.0.0, not
+classes and every `@wp.kernel` they launch are imported UNMODIFIED from $AERIAL_GYM_REFERENCE; `warp` itself (warp-lang 1.0.0, not
 installable) is the interpreter stub of tests/golden/_warp_stub.py, whose one stand-in is the mesh query (brute-force closest hit).
 Pinned by these fixtures (SURVEY 8 rows b1-b7): camera matrices and LiDAR ray table (b6), sensor pose composition (b7), ray
 generation, depth-vs-range multiplier, far plane, miss values, segmentation lookup, point-cloud and normal frames, stereo logic

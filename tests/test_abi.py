@@ -1,4 +1,4 @@
-"""CPU-side checks of the drop-in boundary: the C-ABI library builds for sm_100a, loads, exports
+"""CPU-side checks of the drop-in boundary: the C-ABI library builds for sm_90a (H100), loads, exports
 every symbol include/aerial_gym_b200.h declares, and the ctypes structs match its layout.
 No compute call is made (no GPU here)."""
 import ctypes
@@ -34,10 +34,10 @@ def test_struct_layout_matches(lib):
     assert lib.agx_sizeof(2) == ctypes.sizeof(_lib.AgxHp1ResetDraws)
 
 
-def test_built_for_sm100a_only():
-    out = subprocess.run(["cuobjdump", "--list-elf", _build.LIB], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
-    assert all("sm_100a" in line for line in out.splitlines() if "sm_" in line)
+def test_built_for_sm90a_only():
+    out = subprocess.run([_build.cuda_tool("cuobjdump"), "--list-elf", _build.LIB], capture_output=True, text=True).stdout
+    assert "sm_90a" in out
+    assert all("sm_90a" in line for line in out.splitlines() if "sm_" in line)
 
 
 def test_argument_validation_without_gpu(lib):

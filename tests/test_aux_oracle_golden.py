@@ -56,7 +56,7 @@ def test_imu_matches_reference():
 
 def test_vae_encoder_equals_reference_encoder():
     """utils/vae_encoder.py loads the reference checkpoint and reproduces the reference encoder bit for bit
-    (runs only where /root/reference is mounted: the 44 MB checkpoint does not travel)."""
+    (runs only where AERIAL_GYM_REFERENCE names a reference checkout: the 44 MB checkpoint is not part of this repository)."""
     import contextlib
     import io
     import sys

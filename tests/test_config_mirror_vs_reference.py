@@ -1,5 +1,5 @@
 """The host-side config mirror against the REFERENCE'S OWN config classes, field by field (this container only: the test
-skips where /root/reference does not exist, e.g. on the GPU box).  Paths into the resource tree and the nested sensor config
+skips unless AERIAL_GYM_REFERENCE names a checkout of the reference).  Paths into the resource tree and the nested sensor config
 classes of robot configs (compared on their own) are excluded; everything else must be equal."""
 import importlib
 import inspect

@@ -1,8 +1,8 @@
 """The multi-GPU step loop's launch / residency protocol (DESIGN section 9) as an exhaustively explored model (tests/_protocol_model.py):
-the three failures the B200s showed in round 2 are reachable deadlocks of the earlier designs, and the shipped design (ring gate in front
+the three failures seen on hardware are reachable deadlocks of the earlier designs, and the shipped design (ring gate in front
 of the step, one-warp ready gate in front of the push) has none -- under an adversarial CTA scheduler -- as long as the GPU holds one
 step grid plus one ready gate per ring slot, whatever the number and the footprint of the push CTAs.  Abstract slots, no timing: the
-hardware evidence is in profiles/ (gather_bench_*, p2p_2gpu_r2c_ring_backpressure_deadlock.log) and tests/test_multi_gpu.py."""
+hardware check is tests/test_multi_gpu.py."""
 import itertools
 
 import pytest
@@ -22,7 +22,7 @@ def test_unprotected_ring_is_unsafe():
 
 
 def test_lesson_1_in_kernel_back_pressure_deadlocks():
-    """profiles/p2p_2gpu_r2c_ring_backpressure_deadlock.log: the tiles of step T+ring spin for push T while they and their chained successor
+    """the first multi-GPU design: the tiles of step T+ring spin for push T while they and their chained successor
     hold every CTA slot, so the push never becomes resident.  Safe, but not live unless the GPU holds several whole step grids."""
     p, _, dead, bad = explore(steps=5, tiles=2, slots=4, ring=2, push_ctas=1, design="backpressure")
     assert not bad and dead
@@ -56,7 +56,7 @@ def test_lesson_3_spinning_pushes_are_not_free_even_when_they_fit_on_paper():
                                                                if c[2] * c[3] <= c[0] + c[1]])
 def test_shipped_design_is_live_and_safe_with_a_reserve_of_one_slot_per_ring_slot(tiles, ring, push_ctas, push_weight):
     """every step rare (the worst case), adversarial scheduler: no deadlock and no overwrite with slots = tiles + ring, for every push
-    shape that fits the GPU by itself; and the bound is tight (csrc/hp1.cu: kCoopReserve = 96 slots against a ring of 4)"""
+    shape that fits the GPU by itself; and the bound is tight (csrc/hp1.cu: kCoopReserve = 32 slots against a ring of 4)"""
     steps = 2 * ring + 1
     rare = set(range(1, steps + 1))
     _, states, dead, bad = explore(steps=steps, tiles=tiles, slots=tiles + ring, ring=ring, push_ctas=push_ctas, push_weight=push_weight,

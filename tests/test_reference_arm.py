@@ -10,7 +10,8 @@ import sys
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-_HAVE = os.path.isdir(os.path.join(ROOT, "baseline", "_ref", "aerial_gym", "registry")) or os.path.isdir("/root/reference/aerial_gym")
+_REF = os.environ.get("AERIAL_GYM_REFERENCE", "")
+_HAVE = os.path.isdir(os.path.join(ROOT, "baseline", "_ref", "aerial_gym", "registry")) or bool(_REF and os.path.isdir(os.path.join(_REF, "aerial_gym")))
 pytestmark = pytest.mark.skipif(not _HAVE, reason="reference not staged (baseline/_ref)")
 
 

@@ -2,7 +2,7 @@
 compat.install() on the CPU twins (tests/_cpu_stack.py).  Only three textual substitutions are made before exec:
 "cuda:0" -> "cpu" (no GPU here), the loop counts (10,000 steps -> a few dozen) and nothing else.  What this pins: every attribute
 path, registry name, keyword and call the scripts use exists with the reference's meaning (SURVEY 8b "who calls").
-Needs /root/reference (this container only): skipped elsewhere."""
+Needs a reference checkout named by AERIAL_GYM_REFERENCE: skipped elsewhere."""
 import os
 import re
 import sys
@@ -10,7 +10,7 @@ import sys
 import pytest
 import torch
 
-EX = "/root/reference/aerial_gym/examples"
+EX = os.path.join(os.environ.get("AERIAL_GYM_REFERENCE", ""), "aerial_gym/examples")
 pytestmark = pytest.mark.skipif(not os.path.isdir(EX), reason="reference checkout not present")
 
 from ._cpu_stack import cpu_stack  # noqa: E402

@@ -12,7 +12,7 @@ The reference ships three rl_games checkpoints for rigid-body tasks under exampl
 Bar: every env converges to its setpoint from the random reset state and holds it (no crash, no divergence); the per-episode return is
 compared with the checkpoint's own `last_mean_rewards` for information only (the checkpoints predate the current reward functions).
 Not a parity proof -- a controller tolerates model error -- but a wrong mass / inertia / thrust map / sign would show here.
-Needs /root/reference (this container only)."""
+Needs a reference checkout named by AERIAL_GYM_REFERENCE: skipped elsewhere."""
 import contextlib
 import io
 import os
@@ -21,7 +21,7 @@ import sys
 import pytest
 import torch
 
-NETS = "/root/reference/aerial_gym/examples/rl_games_example/networks"
+NETS = os.path.join(os.environ.get("AERIAL_GYM_REFERENCE", ""), "aerial_gym/examples/rl_games_example/networks")
 pytestmark = pytest.mark.skipif(not os.path.isdir(NETS), reason="reference checkout not present")
 
 from ._cpu_stack import cpu_stack  # noqa: E402

@@ -7,7 +7,7 @@
   * rl_training/cleanrl/ppo_continuous_action.py -- the whole script, __main__ included: two PPO updates on position_setpoint_task;
   * rl_training/sample_factory/.../train_aerialgym.py -- its AerialGymVecEnv class (lifted out by name; sample_factory is not
                                              installed), reset / step through it.
-Needs /root/reference (this container only): skipped elsewhere."""
+Needs a reference checkout named by AERIAL_GYM_REFERENCE: skipped elsewhere."""
 import ast
 import os
 import sys
@@ -17,7 +17,7 @@ import numpy as np
 import pytest
 import torch
 
-RL = "/root/reference/aerial_gym/rl_training"
+RL = os.path.join(os.environ.get("AERIAL_GYM_REFERENCE", ""), "aerial_gym/rl_training")
 pytestmark = pytest.mark.skipif(not os.path.isdir(RL), reason="reference checkout not present")
 
 from ._cpu_stack import cpu_stack  # noqa: E402

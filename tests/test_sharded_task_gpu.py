@@ -66,7 +66,7 @@ def test_sharded_navigation_task_loopback():
     shard.close()
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs >= 2 GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs >= 2 GPUs")
 def test_sharded_position_task_two_ranks_equals_nccl():
     env = dict(os.environ, NCCL_DEBUG="WARN")
     r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",

@@ -1,5 +1,5 @@
 """utils/math.py mirror against the REFERENCE'S OWN utils/math.py on random inputs, function by function (this container only: the
-test skips where /root/reference does not exist).  Same names, same arguments, same values."""
+test skips unless AERIAL_GYM_REFERENCE names a checkout of the reference).  Same names, same arguments, same values."""
 import inspect
 import os
 import sys

@@ -4,7 +4,7 @@ LiDARNavigationTask end to end (env_with_lidar_nav_obstacles: 91 boxes, magpie, 
 
 (Named test_zz_*: these kernels were written after the round's GPU budget was spent -- their arithmetic and indexing
 are verified on CPU by tests/test_lidar_nav_cpu.py through the host shadow build -- so they run after every test that
-has already been green on a B200.)"""
+has already been green on a GPU.)"""
 import ctypes as C
 import os
 

@@ -1,10 +1,10 @@
-"""Round-2 measurement of the kernels written without a GPU in round 1 (not part of bench.py's contract line):
+"""Timing of the small kernels around the two hot paths (not part of bench.py's contract line):
 
     python tools/bench_aux.py [--envs 4096] [--iters 200]          # one JSON line per kernel on stdout
 
 Each kernel is timed with CUDA events on torch's current stream after 10 warm-up launches, inputs rotated over enough replicas to
-exceed the 126 MB L2; `achieved` = algorithmic bytes (DESIGN 6, "Kernels written after the GPU budget was spent") / mean launch time,
-`frac` against MEASURED_PEAKS.json's HBM figure (fallback 6569 GB/s, the round-1 measurement)."""
+exceed the H100's 50 MB L2; `achieved` = algorithmic bytes (DESIGN 6, "Kernels written after the GPU budget was spent") / mean launch time,
+`frac` against MEASURED_PEAKS.json's HBM figure (fallback 3350 GB/s, the H100 SXM data sheet)."""
 import argparse
 import ctypes as C
 import json
@@ -26,7 +26,7 @@ def peak_gbs():
                 return float(d[k]), f"MEASURED_PEAKS.json {k}"
     except Exception:  # noqa: BLE001
         pass
-    return 6569.0, "round-1 measurement (fallback)"
+    return 3350.0, "H100 SXM data sheet (fallback)"
 
 
 def timeit(fn, reps, iters):

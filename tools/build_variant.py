@@ -43,7 +43,7 @@ def main(argv):
                     print(unit, line.strip())
         objs.append(obj)
     lib = os.path.join(ROOT, "tools", "dbg", f"libagx_{name}.so")
-    subprocess.run([_build._nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", lib] + objs, check=True)
+    subprocess.run([_build._nvcc(), "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", lib] + objs, check=True)
     print("built", lib)
 
 

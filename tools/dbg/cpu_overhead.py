@@ -1,5 +1,6 @@
+import os
 import sys, time, torch
-sys.path.insert(0, '/root/repo')
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 from aerial_gym_simulator_b200.hp1 import Hp1Engine, MultirotorSpec
 dev = torch.device("cuda:0")
 N = 65536

@@ -1,6 +1,7 @@
 """1-GPU loopback timing of the chained steps with / without the observation gather attached (emulated world: pushes go to local buffers)."""
+import os
 import sys, torch
-sys.path.insert(0, '/root/repo')
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 from aerial_gym_simulator_b200.distributed import PipelinedObsGather
 from aerial_gym_simulator_b200.hp1 import Hp1Engine, MultirotorSpec
 from aerial_gym_simulator_b200 import _lib

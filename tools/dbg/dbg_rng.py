@@ -1,5 +1,6 @@
+import os
 import torch, sys
-sys.path.insert(0,'/root/repo')
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 import aerial_gym_simulator_b200.task
 from aerial_gym_simulator_b200.registry.task_registry import task_registry
 cfg = task_registry.get_task_config("position_setpoint_task")

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Fly the three rigid-body rl_games checkpoints the reference ships (examples/rl_games_example/networks/*.pth, trained in Isaac Gym)
 on this package's simulator and print a table: final hover error, crashes, per-episode return next to the checkpoint's own
-`last_mean_rewards`.  Build container only (needs /root/reference).  --device cpu runs on the CPU twins of tests/_cpu_stack.py (host
+`last_mean_rewards`.  Needs a reference checkout (AERIAL_GYM_REFERENCE).  --device cpu runs on the CPU twins of tests/_cpu_stack.py (host
 shadow of the device code); --device cuda:0 on the real engine.
 
     python tools/fly_reference_policies.py [--device cpu] [--envs 256] > profiles/reference_policies_r1.md
@@ -17,7 +17,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-NETS = "/root/reference/aerial_gym/examples/rl_games_example/networks"
+NETS = os.path.join(os.environ.get("AERIAL_GYM_REFERENCE", ""), "aerial_gym/examples/rl_games_example/networks")
 CASES = [("position_setpoint_task", "attitude_policy.pth"), ("position_setpoint_task_sim2real", "vel_control_lmf2_direct.pth"),
          ("position_setpoint_task_acceleration_sim2real", "acc_command_2_multiplier_disturbance.pth")]
 

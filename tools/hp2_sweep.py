@@ -1,5 +1,5 @@
 """HP2 throughput on the BASELINE.json sensor configs (synthetic randomly posed box scenes).
-Prints one JSON line per config.  Run on a B200: python tools/hp2_sweep.py [--quick]"""
+Prints one JSON line per config.  Run on an H100: python tools/hp2_sweep.py [--quick]"""
 import argparse
 import json
 import os

@@ -3,7 +3,7 @@
 device functions of csrc/*_core.cuh compiled for the host).  An out-of-bounds index, a misaligned vector access or signed overflow
 in that text shows up here without a GPU; compute-sanitizer on the real kernels covers the thread mapping (profiles/sanitizer_*).
 
-    python tools/shadow_sanitize.py [-k EXPR]          # writes profiles/shadow_sanitizers_<tag>.log (tag: --tag, default r1)
+    python tools/shadow_sanitize.py [-k EXPR]          # writes profiles/shadow_sanitizers_<tag>.log (tag: --tag, default local; git-ignored)
 """
 import argparse
 import os
@@ -21,7 +21,7 @@ def gcc_file(name):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("-k", default="shadow or cpu or host_stack")
-    ap.add_argument("--tag", default="r1")
+    ap.add_argument("--tag", default="local")
     a = ap.parse_args()
     env = dict(os.environ, AGX_SHADOW_FLAGS=FLAGS)
     # build WITHOUT the preload (nvcc itself must not run under ASan)

@@ -1,6 +1,6 @@
 """Re-author the robot / obstacle descriptions the hot paths need as minimal URDFs.
 
-    python tools/strip_resources.py            (build container only: reads /root/reference/resources)
+    python tools/strip_resources.py            (reads $AERIAL_GYM_REFERENCE/resources)
 
 For each source URDF only the physical facts are kept -- link names, inertials, fixed-joint
 origins, box geometry of visuals/collisions -- re-serialised from the parsed model (no meshes,
@@ -14,7 +14,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from aerial_gym_simulator_b200 import urdf  # noqa: E402
 
-SRC = "/root/reference/resources"
+SRC = os.path.join(os.environ.get("AERIAL_GYM_REFERENCE", ""), "resources")
 DST = os.path.join(ROOT, "aerial_gym_simulator_b200", "resources")
 
 

@@ -1,4 +1,4 @@
-"""Summarise an .ncu-rep (read here, no GPU needed) into profiles/<name>.md:
+"""Summarise an .ncu-rep (read here, no GPU needed) into the given .md file:
 duration, DRAM bytes, throughput %, registers, occupancy, top stall reasons."""
 import csv
 import io
