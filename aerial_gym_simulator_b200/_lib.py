@@ -107,7 +107,12 @@ class AgxHp2Scene(C.Structure):
         ("tmpl_tri_offset", fp), ("tmpl_tris", fp), ("tmpl_seg_base", fp), ("tmpl_seg_mask", fp),
         ("obj_pose", fp), ("obj_template", fp), ("obj_seg_counter", fp), ("bounds_min", fp), ("bounds_max", fp),
         ("tris", fp), ("nodes", fp), ("leaf_object", fp), ("face_offset", fp), ("tmpl_obb", fp), ("obb", fp),
+        ("num_meshes", C.c_int32), ("mesh_tris_per_env", C.c_int32), ("mesh_nodes_per_env", C.c_int32), ("mesh_pad_", C.c_int32),
+        ("tmpl_mesh", fp), ("mesh_tri_offset", fp), ("mesh_tris", fp), ("mesh_tri_index", fp), ("mesh_seg", fp),
+        ("mesh_node_offset", fp), ("mesh_topo", fp), ("mesh_levels", fp), ("obj_mesh_slot", fp),
+        ("mesh_world_tris", fp), ("mesh_world_nodes", fp),
     ]
+BLAS_MAX_DEPTH = 24  # AGX_HP2_BLAS_MAX_DEPTH
 
 
 class AgxHp2Sensor(C.Structure):

@@ -10,6 +10,8 @@
 //                          Per ray: sensor pose compose, ray generation, stack traversal,
 //                          Moller-Trumbore on the leaf's triangle slab, fused range-limit /
 //                          normalise epilogue, coalesced row stores.
+//   mesh objects          : (URDF <mesh> / <sphere>) one top-level leaf each, over a per-template BLAS whose boxes the scene
+//                          update refits in world space; the cast walks it per ray (hp2_cast_kernel<SMEM, false, true>).
 //
 // This unit is compiled with -fmad=false and every fusable multiply-add on the RESULT path is an
 // explicit fmaf(): the arithmetic is then bit-reproducible by oracle/hp2_oracle.c
@@ -21,6 +23,8 @@
 #include <cuda_runtime.h>
 #include <float.h>
 #include <stdint.h>
+
+#include <type_traits>
 
 #include "../../include/aerial_gym_b200.h"
 #include "agx_common.cuh"
@@ -138,12 +142,41 @@ hp2_update_scene_kernel(const __grid_constant__ AgxHp2Scene sc, const uint8_t* _
         float4* dst = reinterpret_cast<float4*>(tris + (size_t)i * kTriFloats);
         dst[0] = o0; dst[1] = o1; dst[2] = o2;
     }
+    const int M = sc.num_meshes;
+    const int32_t* slot = M ? sc.obj_mesh_slot + (size_t)e * K * 2 : nullptr;
+    if (M) {  // mesh objects: world triangles into the env's mesh slab, in BLAS leaf order (same arithmetic as pass A)
+        float* wt = sc.mesh_world_tris + (size_t)e * sc.mesh_tris_per_env * kTriFloats;
+        for (int k = 0; k < K; ++k) {
+            if (slot[2 * k] < 0) continue;
+            const float* p = sc.obj_pose + ((size_t)e * K + k) * sc.obj_pose_stride;
+            v3 t{p[0], p[1], p[2]};
+            q4 q{p[3], p[4], p[5], p[6]};
+            const int m = sc.tmpl_mesh[sc.obj_template[(size_t)e * K + k]];
+            const int f0 = sc.mesh_tri_offset[m], n = sc.mesh_tri_offset[m + 1] - f0;
+            const int seg = sc.mesh_seg[2 * m] + sc.obj_seg_counter[(size_t)e * K + k] * sc.mesh_seg[2 * m + 1];
+            for (int i = tid; i < n; i += nt) {
+                const float* tv = sc.mesh_tris + (size_t)(f0 + i) * 9;
+                v3 wa = quat_apply(q, v3{tv[0], tv[1], tv[2]});
+                v3 wb = quat_apply(q, v3{tv[3], tv[4], tv[5]});
+                v3 wc = quat_apply(q, v3{tv[6], tv[7], tv[8]});
+                wa.x += t.x; wa.y += t.y; wa.z += t.z;
+                wb.x += t.x; wb.y += t.y; wb.z += t.z;
+                wc.x += t.x; wc.y += t.y; wc.z += t.z;
+                v3 e1 = sub3(wb, wa), e2 = sub3(wc, wa);
+                float4* dst = reinterpret_cast<float4*>(wt + (size_t)(slot[2 * k] + i) * kTriFloats);
+                dst[0] = make_float4(wa.x, wa.y, wa.z, __int_as_float(seg));
+                dst[1] = make_float4(e1.x, e1.y, e1.z, __int_as_float(sc.mesh_tri_index[f0 + i]));
+                dst[2] = make_float4(e2.x, e2.y, e2.z, 0.f);
+            }
+        }
+    }
     if (sc.face_offset && tid == 0) {
         int acc = 0;
         for (int k = 0; k < K; ++k) {
             sc.face_offset[(size_t)e * K + k] = acc;
             int tm = sc.obj_template[(size_t)e * K + k];
             acc += min(L, sc.tmpl_tri_offset[tm + 1] - sc.tmpl_tri_offset[tm]);
+            if (M && slot[2 * k] >= 0) acc += sc.mesh_tri_offset[sc.tmpl_mesh[tm] + 1] - sc.mesh_tri_offset[sc.tmpl_mesh[tm]];
         }
     }
     if (sc.obb) {  // world-frame oriented boxes of box-shaped objects (culling aid)
@@ -164,8 +197,60 @@ hp2_update_scene_kernel(const __grid_constant__ AgxHp2Scene sc, const uint8_t* _
         }
     }
     __syncthreads();  // slabs of this CTA are read back below (same CTA wrote them)
-    // pass B: object AABBs from the slabs just written
+    if (M) {  // refit the BLAS boxes of the mesh objects bottom-up, one depth level at a time (the reference's mesh.refit())
+        const float* wt = sc.mesh_world_tris + (size_t)e * sc.mesh_tris_per_env * kTriFloats;
+        float* wn = sc.mesh_world_nodes + (size_t)e * sc.mesh_nodes_per_env * kNodeFloats;
+        for (int d = AGX_HP2_BLAS_MAX_DEPTH - 1; d >= 0; --d) {
+            for (int k = 0; k < K; ++k) {
+                if (slot[2 * k] < 0) continue;
+                const int m = sc.tmpl_mesh[sc.obj_template[(size_t)e * K + k]];
+                const int* lv = sc.mesh_levels + (size_t)m * (AGX_HP2_BLAS_MAX_DEPTH + 1);
+                const int2* topo = reinterpret_cast<const int2*>(sc.mesh_topo) + sc.mesh_node_offset[m];
+                const float* ot = wt + (size_t)slot[2 * k] * kTriFloats;
+                float* on = wn + (size_t)slot[2 * k + 1] * kNodeFloats;
+                for (int i = lv[d] + tid; i < lv[d + 1]; i += nt) {
+                    const int2 tp = topo[i];
+                    float lo[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, hi[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
+                    if (tp.y > 0) {
+                        for (int s = tp.x; s < tp.x + tp.y; ++s) {
+                            const float4* src = reinterpret_cast<const float4*>(ot + (size_t)s * kTriFloats);
+                            float4 a = src[0], b = src[1], c = src[2];
+                            float vx[3] = {a.x, a.x + b.x, a.x + c.x}, vy[3] = {a.y, a.y + b.y, a.y + c.y}, vz[3] = {a.z, a.z + b.z, a.z + c.z};
+#pragma unroll
+                            for (int j = 0; j < 3; ++j) {
+                                lo[0] = fminf(lo[0], vx[j]); hi[0] = fmaxf(hi[0], vx[j]);
+                                lo[1] = fminf(lo[1], vy[j]); hi[1] = fmaxf(hi[1], vy[j]);
+                                lo[2] = fminf(lo[2], vz[j]); hi[2] = fmaxf(hi[2], vz[j]);
+                            }
+                        }
+#pragma unroll
+                        for (int j = 0; j < 3; ++j) {
+                            float pad = kAabbPad + 1e-6f * fmaxf(fabsf(lo[j]), fabsf(hi[j]));
+                            lo[j] -= pad;
+                            hi[j] += pad;
+                        }
+                    } else {
+                        const float* a = on + (size_t)tp.x * kNodeFloats;
+                        const float* b = a + kNodeFloats;
+#pragma unroll
+                        for (int j = 0; j < 3; ++j) { lo[j] = fminf(a[j], b[j]); hi[j] = fmaxf(a[4 + j], b[4 + j]); }
+                    }
+                    float4* dst = reinterpret_cast<float4*>(on + (size_t)i * kNodeFloats);
+                    dst[0] = make_float4(lo[0], lo[1], lo[2], 0.f);
+                    dst[1] = make_float4(hi[0], hi[1], hi[2], 0.f);
+                }
+            }
+            __syncthreads();
+        }
+    }
+    // pass B: object AABBs from the slabs just written (a mesh object: its BLAS root box, already padded)
     for (int k = tid; k < K; k += nt) {
+        if (M && slot[2 * k] >= 0) {
+            const float* rn = sc.mesh_world_nodes + ((size_t)e * sc.mesh_nodes_per_env + slot[2 * k + 1]) * kNodeFloats;
+#pragma unroll
+            for (int j = 0; j < 3; ++j) { s_olo[k * 3 + j] = rn[j]; s_ohi[k * 3 + j] = rn[4 + j]; }
+            continue;
+        }
         float lo[3] = {FLT_MAX, FLT_MAX, FLT_MAX}, hi[3] = {-FLT_MAX, -FLT_MAX, -FLT_MAX};
         int tm = sc.obj_template[(size_t)e * K + k];
         int n = min(L, sc.tmpl_tri_offset[tm + 1] - sc.tmpl_tri_offset[tm]);
@@ -301,8 +386,32 @@ __device__ __forceinline__ void tma_bulk_g2s(void* dst, const void* src, uint32_
 
 struct Hit {
     float t;
-    int tri;
+    int tri;   // tie-break index: obj * L + slot, or (scenes with mesh objects) the face id in the env's concatenated mesh
 };
+struct MeshHit : Hit {
+    int slab;  // >= 0 cluster slab index, < 0 mesh slab -(slab + 1)
+};
+
+// per-env view of the mesh objects of a scene (num_meshes > 0)
+struct MeshCtx {
+    const int32_t* slot;          // [K,2] first triangle / node in the env's mesh slabs, -1 = cluster object
+    const int32_t* obj_template;  // [K]
+    const int32_t* face_offset;   // [K]
+    const float* tris;            // env mesh slab
+    const float* nodes;           // env BLAS boxes
+};
+__device__ __forceinline__ MeshCtx mesh_ctx(const AgxHp2Scene& sc, int e) {
+    const int K = sc.num_objects;
+    return MeshCtx{sc.obj_mesh_slot + (size_t)e * K * 2, sc.obj_template + (size_t)e * K, sc.face_offset + (size_t)e * K,
+                   sc.mesh_world_tris + (size_t)e * sc.mesh_tris_per_env * kTriFloats,
+                   sc.mesh_world_nodes + (size_t)e * sc.mesh_nodes_per_env * kNodeFloats};
+}
+// triangle slab of a hit
+template <bool MESH, class H>
+__device__ __forceinline__ const float* hit_slab(const H& h, const float* tris, const MeshCtx& mc) {
+    if constexpr (MESH) return h.slab >= 0 ? tris + (size_t)h.slab * kTriFloats : mc.tris + (size_t)(-h.slab - 1) * kTriFloats;
+    else return tris + (size_t)h.tri * kTriFloats;
+}
 
 // Moller-Trumbore on one triangle slab (bit contract with oracle closest_hit)
 __device__ __forceinline__ void tri_test(const float4* __restrict__ tp, int tri_index, v3 o, v3 d, float max_t, Hit& best) {
@@ -368,11 +477,55 @@ __device__ __forceinline__ bool obb_may_hit(const float* __restrict__ b, v3 o, v
     return tmin <= tmax + 1e-5f * (1.0f + fabsf(tmax));
 }
 
-template <bool SMEM>
-__device__ __forceinline__ Hit traverse(const float* __restrict__ nodes, const int32_t* __restrict__ leaf_obj,
-                                        const float* __restrict__ tris, const float* __restrict__ obb, int P, int L, v3 o, v3 d,
-                                        float max_t) {
-    Hit best{max_t, 0x7fffffff};
+// one mesh object: walk its BLAS in world space (L2 reads); keys are face ids, so ties go to the lowest file-order index
+__device__ __forceinline__ void mesh_object_test(const AgxHp2Scene& sc, const MeshCtx& mc, int obj, v3 o, v3 d, v3 inv, float max_t,
+                                                 MeshHit& best) {
+    const int ts = mc.slot[2 * obj];
+    const int m = sc.tmpl_mesh[mc.obj_template[obj]];
+    const int2* topo = reinterpret_cast<const int2*>(sc.mesh_topo) + sc.mesh_node_offset[m];
+    const float* nodes = mc.nodes + (size_t)mc.slot[2 * obj + 1] * kNodeFloats;
+    const float4* tp = reinterpret_cast<const float4*>(mc.tris + (size_t)ts * kTriFloats);
+    const int fo = mc.face_offset[obj];
+    int stack[AGX_HP2_BLAS_MAX_DEPTH];
+    int sp = 0, node = 0;  // the root box is the object's top-level leaf box, already tested
+    while (true) {
+        const int2 t = topo[node];
+        if (t.y > 0) {
+            for (int s = t.x; s < t.x + t.y; ++s) {
+                const int before = best.tri;
+                tri_test(tp + 3 * s, fo + __float_as_int(tp[3 * s + 1].w), o, d, max_t, best);
+                if (best.tri != before) best.slab = -(ts + s) - 1;
+            }
+            if (sp == 0) break;
+            node = stack[--sp];
+            continue;
+        }
+        const int c0 = t.x, c1 = c0 + 1;
+        const float t0 = aabb_entry(nodes + (size_t)c0 * kNodeFloats, o, inv, best.t);
+        const float t1 = aabb_entry(nodes + (size_t)c1 * kNodeFloats, o, inv, best.t);
+        if (t0 >= 0.0f && t1 >= 0.0f) {
+            if (t0 <= t1) { stack[sp++] = c1; node = c0; }
+            else { stack[sp++] = c0; node = c1; }
+        } else if (t0 >= 0.0f) {
+            node = c0;
+        } else if (t1 >= 0.0f) {
+            node = c1;
+        } else {
+            if (sp == 0) break;
+            node = stack[--sp];
+        }
+    }
+}
+
+// MESH: the scene has mesh objects (sc, mc given): their leaves walk the object's BLAS, cluster leaves key their triangles
+// by face id so that ties resolve as in the env's concatenated mesh
+template <bool SMEM, bool MESH = false>
+__device__ __forceinline__ auto traverse(const float* __restrict__ nodes, const int32_t* __restrict__ leaf_obj,
+                                         const float* __restrict__ tris, const float* __restrict__ obb, int P, int L, v3 o, v3 d,
+                                         float max_t, const AgxHp2Scene* sc = nullptr, const MeshCtx* mc = nullptr) {
+    typename std::conditional<MESH, MeshHit, Hit>::type best{};
+    best.t = max_t;
+    best.tri = 0x7fffffff;
     v3 inv{1.0f / d.x, 1.0f / d.y, 1.0f / d.z};
     int stack[24];
     int sp = 0;
@@ -385,6 +538,20 @@ __device__ __forceinline__ Hit traverse(const float* __restrict__ nodes, const i
     while (true) {
         if (node >= P - 1) {  // leaf
             int obj = leaf_obj[node - (P - 1)];
+            if constexpr (MESH) {
+                if (obj >= 0 && mc->slot[2 * obj] >= 0) {
+                    mesh_object_test(*sc, *mc, obj, o, d, inv, max_t, best);
+                } else if (obj >= 0) {
+                    const float4* tp = reinterpret_cast<const float4*>(tris + (size_t)obj * L * kTriFloats);
+                    const int fo = mc->face_offset[obj];
+                    for (int s = 0; s < L; ++s) {
+                        const int before = best.tri;
+                        tri_test(tp + 3 * s, fo + s, o, d, max_t, best);
+                        if (best.tri != before) best.slab = obj * L + s;
+                    }
+                }
+                obj = -1;
+            }
             if (obj >= 0) {
                 bool test = true;
                 if (obb) {
@@ -666,6 +833,40 @@ __device__ __forceinline__ float point_tri_dist2(v3 p, v3 a, v3 ab, v3 ac) {
     return dot3(d, d);
 }
 
+// one mesh object: descend its BLAS with the same sphere/box test as the top level; min is order-independent, so the
+// result is the oracle's min over the object's triangles within reach
+__device__ __noinline__ float mesh_sphere_min(const AgxHp2Scene& sc, const MeshCtx& mc, int obj, v3 c, float search, float best) {
+    const int m = sc.tmpl_mesh[mc.obj_template[obj]];
+    const int2* topo = reinterpret_cast<const int2*>(sc.mesh_topo) + sc.mesh_node_offset[m];
+    const float* nodes = mc.nodes + (size_t)mc.slot[2 * obj + 1] * kNodeFloats;
+    const float4* tp = reinterpret_cast<const float4*>(mc.tris + (size_t)mc.slot[2 * obj] * kTriFloats);
+    int stack[AGX_HP2_BLAS_MAX_DEPTH];
+    int sp = 0, node = 0;
+    while (true) {
+        const float* nd = nodes + (size_t)node * kNodeFloats;
+        float dx = fmaxf(fmaxf(nd[0] - c.x, c.x - nd[4]), 0.0f);
+        float dy = fmaxf(fmaxf(nd[1] - c.y, c.y - nd[5]), 0.0f);
+        float dz = fmaxf(fmaxf(nd[2] - c.z, c.z - nd[6]), 0.0f);
+        float box_d2 = dx * dx + dy * dy + dz * dz;
+        if (box_d2 <= fminf(best, search) * 1.0001f + 1e-6f) {  // culling only, as at the top level
+            const int2 t = topo[node];
+            if (t.y > 0) {
+                for (int s = t.x; s < t.x + t.y; ++s) {
+                    float4 a = tp[3 * s], b = tp[3 * s + 1], cc = tp[3 * s + 2];
+                    best = fminf(best, point_tri_dist2(c, v3{a.x, a.y, a.z}, v3{b.x, b.y, b.z}, v3{cc.x, cc.y, cc.z}));
+                }
+            } else {
+                stack[sp++] = t.x + 1;
+                node = t.x;
+                continue;
+            }
+        }
+        if (sp == 0) break;
+        node = stack[--sp];
+    }
+    return best;
+}
+
 // one thread per env: BVH descent with a sphere/AABB overlap test, exact min distance over the
 // triangles of every leaf the sphere of the CURRENT best radius can reach
 __global__ void __launch_bounds__(128)
@@ -697,7 +898,9 @@ hp2_collide_kernel(const __grid_constant__ AgxHp2Scene sc, const float* __restri
         if (reach) {
             if (node >= P - 1) {
                 int obj = leaf[node - (P - 1)];
-                if (obj >= 0) {
+                if (obj >= 0 && sc.num_meshes && sc.obj_mesh_slot[((size_t)e * K + obj) * 2] >= 0) {
+                    best = mesh_sphere_min(sc, mesh_ctx(sc, e), obj, c, search, best);
+                } else if (obj >= 0) {
                     const float4* tp = reinterpret_cast<const float4*>(tris + (size_t)obj * L * kTriFloats);
                     for (int s = 0; s < L; ++s) {
                         float4 a = tp[3 * s], b = tp[3 * s + 1], cc = tp[3 * s + 2];
@@ -734,7 +937,8 @@ constexpr int kCastThreads = 256;
 #ifndef AGX_CAST_MIN_BLOCKS
 #define AGX_CAST_MIN_BLOCKS 4
 #endif
-template <bool SMEM, bool TILE = false>
+// MESH: scene with mesh objects (num_meshes > 0; per-ray traversal only, TILE = false)
+template <bool SMEM, bool TILE = false, bool MESH = false>
 __global__ void __launch_bounds__(kCastThreads, AGX_CAST_MIN_BLOCKS)
 hp2_cast_kernel(const __grid_constant__ AgxHp2Scene sc, const __grid_constant__ AgxHp2Sensor sn, int rows_per_item,
                 int items_per_image, long long n_items, int rec_cap) {
@@ -776,6 +980,8 @@ hp2_cast_kernel(const __grid_constant__ AgxHp2Scene sc, const __grid_constant__ 
         const int32_t* leaf = g_leaf;
         const float* tris = g_tris;
         const float* obb = g_obb;
+        MeshCtx mc{};
+        if constexpr (MESH) mc = mesh_ctx(sc, e);
         bool fresh_scene = false;  // uniform: this item staged a new scene (its leading barrier also retired the previous item's records)
         if (SMEM) {
             if (e != staged_env) {
@@ -897,13 +1103,13 @@ hp2_cast_kernel(const __grid_constant__ AgxHp2Scene sc, const __grid_constant__ 
                 uv = normalize3(v3{rt[0], rt[1], rt[2]});
                 rd = normalize3(quat_rotate(sq, uv));
             }
-            Hit h;
+            typename std::conditional<MESH, MeshHit, Hit>::type h;
             if constexpr (tile_path) {
                 if (!rec_overflow) h = tile_closest_hit(s_rec, n_rec, tris, L, sp, rd, max_t, lane);
-                else h = traverse<SMEM>(nodes, leaf, tris, obb, P, L, sp, rd, max_t);
+                else h = traverse<SMEM, MESH>(nodes, leaf, tris, obb, P, L, sp, rd, max_t, &sc, &mc);
                 if (!in_image) continue;
             } else {
-                h = traverse<SMEM>(nodes, leaf, tris, obb, P, L, sp, rd, max_t);
+                h = traverse<SMEM, MESH>(nodes, leaf, tris, obb, P, L, sp, rd, max_t, &sc, &mc);
             }
             float dist = AGX_NO_HIT_RAY_VAL;
             int segv = AGX_NO_HIT_SEG_VAL;
@@ -913,7 +1119,7 @@ hp2_cast_kernel(const __grid_constant__ AgxHp2Scene sc, const __grid_constant__ 
                 v3 o{0.f, 0.f, 0.f};
                 int face = -1;
                 if (hit) {
-                    const float4* tp = reinterpret_cast<const float4*>(tris + (size_t)h.tri * kTriFloats);
+                    const float4* tp = reinterpret_cast<const float4*>(hit_slab<MESH>(h, tris, mc));
                     float4 b = tp[1], cc = tp[2];
                     v3 nrm = normalize3(cross3(v3{b.x, b.y, b.z}, v3{cc.x, cc.y, cc.z}));
                     if (sn.normal_in_world_frame) o = nrm;
@@ -921,8 +1127,12 @@ hp2_cast_kernel(const __grid_constant__ AgxHp2Scene sc, const __grid_constant__ 
                         o = v3{dot3(nrm, rd_p), dot3(nrm, cross3(rd_p, v3{0.f, 0.f, 1.f})), dot3(nrm, cross3(rd_p, v3{0.f, 1.f, 0.f}))};
                     else
                         o = normalize3(quat_rotate(q4{-sq.x, -sq.y, -sq.z, sq.w}, nrm));
-                    int obj = h.tri / L;
-                    face = (sc.face_offset ? sc.face_offset[(size_t)e * K + obj] : obj * L) + (h.tri - obj * L);
+                    if constexpr (MESH) {
+                        face = h.tri;
+                    } else {
+                        int obj = h.tri / L;
+                        face = (sc.face_offset ? sc.face_offset[(size_t)e * K + obj] : obj * L) + (h.tri - obj * L);
+                    }
                 }
                 sn.pixels[pix * 3 + 0] = o.x; sn.pixels[pix * 3 + 1] = o.y; sn.pixels[pix * 3 + 2] = o.z;
                 if (sn.seg_pixels) sn.seg_pixels[pix] = face;
@@ -935,11 +1145,11 @@ hp2_cast_kernel(const __grid_constant__ AgxHp2Scene sc, const __grid_constant__ 
                 else ep = v3{sp.x + (rd.x * sn.far_plane) / mult, sp.y + (rd.y * sn.far_plane) / mult, sp.z + (rd.z * sn.far_plane) / mult};
                 v3 dv = sub3(stereo_pos, ep);
                 float dl = sqrtf(dot3(dv, dv));
-                Hit h2 = traverse<SMEM>(nodes, leaf, tris, obb, P, L, ep, normalize3(dv), dl);
+                Hit h2 = traverse<SMEM, MESH>(nodes, leaf, tris, obb, P, L, ep, normalize3(dv), dl, &sc, &mc);
                 const bool visible = h2.tri == 0x7fffffff;
                 if (hit && visible) {
                     dist = h.t * mult;
-                    segv = __float_as_int(tris[(size_t)h.tri * kTriFloats + 3]);
+                    segv = __float_as_int((hit_slab<MESH>(h, tris, mc))[3]);
                 } else if (!hit && visible) {
                     dist = AGX_NO_HIT_RAY_VAL;
                 }
@@ -949,7 +1159,7 @@ hp2_cast_kernel(const __grid_constant__ AgxHp2Scene sc, const __grid_constant__ 
             }
             if (hit) {
                 dist = mult * h.t;
-                segv = __float_as_int(tris[(size_t)h.tri * kTriFloats + 3]);
+                segv = __float_as_int((hit_slab<MESH>(h, tris, mc))[3]);
             }
             if (sn.return_pointcloud) {
                 v3 p;
@@ -993,6 +1203,17 @@ int validate_scene(const AgxHp2Scene* sc) {
     if ((sc->tmpl_obb == nullptr) != (sc->obb == nullptr)) return agx_set_error(AGX_E_INVALID, "tmpl_obb and obb must be given together");
     if ((uintptr_t)sc->obb & 15) return agx_set_error(AGX_E_INVALID, "obb storage must be 16-byte aligned");
     if (((uintptr_t)sc->tris | (uintptr_t)sc->nodes | (uintptr_t)sc->leaf_object) & 15) return agx_set_error(AGX_E_INVALID, "scene storage must be 16-byte aligned");
+    if (sc->num_meshes < 0 || sc->num_meshes > sc->num_templates) return agx_set_error(AGX_E_INVALID, "num_meshes must be in [0, num_templates]");
+    if (sc->num_meshes) {
+        if (!sc->tmpl_mesh || !sc->mesh_tri_offset || !sc->mesh_tris || !sc->mesh_tri_index || !sc->mesh_seg || !sc->mesh_node_offset ||
+            !sc->mesh_topo || !sc->mesh_levels || !sc->obj_mesh_slot || !sc->mesh_world_tris || !sc->mesh_world_nodes)
+            return agx_set_error(AGX_E_NULL, "mesh tables / storage are NULL");
+        if (!sc->face_offset) return agx_set_error(AGX_E_NULL, "a scene with mesh objects needs face_offset");
+        if (sc->mesh_tris_per_env < 1 || sc->mesh_nodes_per_env < 1)
+            return agx_set_error(AGX_E_INVALID, "mesh_tris_per_env and mesh_nodes_per_env must be positive");
+        if (((uintptr_t)sc->mesh_world_tris | (uintptr_t)sc->mesh_world_nodes | (uintptr_t)sc->mesh_topo) & 15)
+            return agx_set_error(AGX_E_INVALID, "mesh storage must be 16-byte aligned");
+    }
     return AGX_OK;
 }
 
@@ -1068,6 +1289,19 @@ int agx_hp2_cast(const AgxHp2Scene* sc, const AgxHp2Sensor* sn, void* stream) {
     size_t smem = scene_smem_bytes(sc->num_objects, sc->leaves_pow2, sc->tris_per_object, sc->obb != nullptr);
     bool use_smem = smem + 1024 <= (size_t)max_smem;
     cudaStream_t st = (cudaStream_t)stream;
+    if (sc->num_meshes) {  // mesh objects: per-ray walk of the top level (staged when it fits) and of each reached BLAS (L2)
+        auto kern = use_smem ? hp2_cast_kernel<true, false, true> : hp2_cast_kernel<false, false, true>;
+        if (!use_smem) smem = 0;
+        rc = agx_check_cuda(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem), "cudaFuncSetAttribute(cast)");
+        if (rc) return rc;
+        int per_sm = 1;
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kCastThreads, smem);
+        if (per_sm < 1) per_sm = 1;
+        long long grid = (long long)sms * per_sm;
+        if (grid > n_items) grid = n_items;
+        kern<<<(int)grid, kCastThreads, smem, st>>>(*sc, *sn, rows_per_item, items_per_image, n_items, 0);
+        return agx_check_launch("hp2_cast_kernel");
+    }
     const bool use_tile = use_smem && sc->leaves_pow2 <= kTileMaxLeaves &&
                           smem + record_smem_bytes(sc->num_objects) + 1024 <= (size_t)max_smem;
     if (use_tile) {  // small staged scenes: warp-per-tile candidate culling, no per-ray BVH walk

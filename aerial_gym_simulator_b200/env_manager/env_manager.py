@@ -224,9 +224,11 @@ class EnvManager:
         gtd["obstacle_linvel"], gtd["obstacle_angvel"] = ast[..., 7:10], ast[..., 10:13]
         lo = np.zeros((N, A, 13), np.float32)
         hi = np.zeros((N, A, 13), np.float32)
-        # templates: every <box> / <cylinder> visual of every distinct URDF; an asset with b parts = b objects sharing its pose
-        # (a box is one part, a tessellated cylinder eleven: urdf.visual_parts)
-        tmpl_index, templates, tmpl_obbs, boxes_of, tmpl_link = {}, [], [], {}, []
+        # templates: every visual of every distinct URDF; an asset with b parts = b objects sharing its pose (a box is one part, a
+        # tessellated cylinder eleven, a <mesh> / <sphere> one mesh object: urdf.visual_parts).  Mesh parts are numbered after
+        # every cluster template (RayScene's mesh_templates).
+        templates, tmpl_obbs, boxes_of, tmpl_link = [], [], {}, []
+        meshes, mesh_link = [], []
         for e in range(N):
             for a, (params, path) in enumerate(per_env[e]):
                 lo[e, a], hi[e, a] = params.min_state_ratio, params.max_state_ratio
@@ -234,7 +236,11 @@ class EnvManager:
                     model = urdf.parse_urdf(path)
                     ids = []
                     for _, link_index, tris, obb in urdf.visual_parts(model, params.use_collision_mesh_instead_of_visual):
-                        tmpl_index[(path, len(ids))] = len(templates)
+                        if obb is None:
+                            ids.append(-1 - len(meshes))
+                            meshes.append(tris)
+                            mesh_link.append(link_index)
+                            continue
                         ids.append(len(templates))
                         templates.append(tris)
                         tmpl_obbs.append(obb)
@@ -244,6 +250,11 @@ class EnvManager:
         gtd["asset_max_state_ratio"].copy_(torch.from_numpy(hi))
         if not self.use_warp:
             return
+        T = len(templates)
+        boxes_of = {p: [t if t >= 0 else T - 1 - t for t in ids] for p, ids in boxes_of.items()}
+        tmpl_link += mesh_link
+        tmpl_obbs += [np.zeros(16, np.float32)] * len(meshes)
+        templates_all = templates + meshes
         nb = [sum(len(boxes_of[p]) for _, p in per_env[e]) for e in range(N)]
         K = max(nb)
         if K == 0:
@@ -251,7 +262,7 @@ class EnvManager:
         obj_t = np.zeros((N, K), np.int32)
         obj_c = np.zeros((N, K), np.int32)
         obj_asset = np.zeros((N, K), np.int64)
-        seg_base, seg_mask = [0] * len(templates), [0] * len(templates)
+        seg_base, seg_mask = [0] * len(templates_all), [0] * len(templates_all)
         seg_ctr = 100  # env_manager.py:147; global across envs like the reference
         for e in range(N):
             k = 0
@@ -276,7 +287,7 @@ class EnvManager:
         self._obj_pose = torch.zeros(N, K, 7, device=dev)
         self.scene = RayScene(templates, seg_base, seg_mask, obj_t, obj_c, self._obj_pose, dev,
                               bounds_min=self.engine.bounds_min, bounds_max=self.engine.bounds_max,
-                              tmpl_obb=np.stack(tmpl_obbs))
+                              tmpl_obb=np.stack(tmpl_obbs), **({"mesh_templates": meshes} if meshes else {}))  # keyword only when used
         # Until the first reset_idx every actor sits where it was created: at the env origin, identity orientation
         # (IGE_env_manager.py: create_actor with the default start pose), the robot among them.  Tasks whose reset() does not reset the
         # sim (NavigationTask.reset, navigation_task.py:162-175) therefore begin in contact: the first step flags a crash and the

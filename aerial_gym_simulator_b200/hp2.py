@@ -59,6 +59,73 @@ def cylinder_triangles(radius: float, length: float, sections: int = 32) -> np.n
     return np.asarray(tris, dtype=np.float32).reshape(-1, 9)
 
 
+def icosphere_triangles(radius: float, subdivisions: int = 3) -> np.ndarray:
+    """[20*4^s,9] object-frame triangles of a URDF <sphere radius/>: what urdfpy obtains from trimesh.creation.icosphere (3
+    subdivisions: 642 vertices, 1280 faces).  Restated from the published construction: the regular icosahedron, each face split
+    into four at its edge midpoints (a, ab, ca | ab, b, bc | ca, bc, c | ab, bc, ca), shared midpoints merged, every vertex
+    projected onto the sphere.  Parity against trimesh's own vertex order unpinned, as for cylinder_triangles."""
+    t = (1.0 + math.sqrt(5.0)) / 2.0
+    v = [[-1, t, 0], [1, t, 0], [-1, -t, 0], [1, -t, 0], [0, -1, t], [0, 1, t], [0, -1, -t], [0, 1, -t],
+         [t, 0, -1], [t, 0, 1], [-t, 0, -1], [-t, 0, 1]]
+    v = [np.asarray(x, np.float64) / np.linalg.norm(x) for x in v]
+    f = [(0, 11, 5), (0, 5, 1), (0, 1, 7), (0, 7, 10), (0, 10, 11), (1, 5, 9), (5, 11, 4), (11, 10, 2), (10, 7, 6), (7, 1, 8),
+         (3, 9, 4), (3, 4, 2), (3, 2, 6), (3, 6, 8), (3, 8, 9), (4, 9, 5), (2, 4, 11), (6, 2, 10), (8, 6, 7), (9, 8, 1)]
+    for _ in range(subdivisions):
+        mid = {}
+
+        def m(i, j):
+            key = (min(i, j), max(i, j))
+            if key not in mid:
+                c = v[i] + v[j]
+                mid[key] = len(v)
+                v.append(c / np.linalg.norm(c))
+            return mid[key]
+
+        nf = []
+        for a, b, c in f:
+            ab, bc, ca = m(a, b), m(b, c), m(c, a)
+            nf += [(a, ab, ca), (ab, b, bc), (ca, bc, c), (ab, bc, ca)]
+        f = nf
+    return (np.asarray(v)[np.asarray(f)] * float(radius)).reshape(-1, 9).astype(np.float32)
+
+
+BLAS_LEAF_TRIS = 4
+
+
+def build_blas(tris) -> dict:
+    """Bottom-level BVH of one mesh template, built once on the host, deterministic: breadth-first binary tree, every node
+    splits its triangles at the median of their centroids along the longest axis of the centroid bounds (stable sort, so ties
+    keep file order), leaves of <= BLAS_LEAF_TRIS triangles.  The median split bounds the depth by log2(n / BLAS_LEAF_TRIS) + 1.
+    Returns order [n] (file index of each leaf-order triangle), topo [N,2] ((first child, 0) internal / (first triangle, count)
+    leaf), levels [AGX_HP2_BLAS_MAX_DEPTH + 1] (nodes of depth d are levels[d]:levels[d+1])."""
+    t = np.asarray(tris, np.float32).reshape(-1, 3, 3).astype(np.float64)
+    n = len(t)
+    if n < 1:
+        raise ValueError("a mesh needs at least one triangle")
+    cent = t.mean(axis=1)
+    order = np.arange(n)
+    nodes, topo, depth = [(0, n, 0)], [], []
+    i = 0
+    while i < len(nodes):
+        a, b, d = nodes[i]
+        depth.append(d)
+        if b - a <= BLAS_LEAF_TRIS:
+            topo.append((a, b - a))
+        else:
+            c = cent[order[a:b]]
+            ax = int(np.argmax(c.max(axis=0) - c.min(axis=0)))
+            order[a:b] = order[a:b][np.argsort(c[:, ax], kind="stable")]
+            mid = a + (b - a) // 2
+            topo.append((len(nodes), 0))
+            nodes += [(a, mid, d + 1), (mid, b, d + 1)]
+        i += 1
+    D = _lib.BLAS_MAX_DEPTH
+    if max(depth) >= D:
+        raise ValueError(f"mesh of {n} triangles: BLAS deeper than {D} levels")
+    levels = np.searchsorted(np.asarray(depth), np.arange(D + 1), side="left").astype(np.int32)
+    return dict(order=order.astype(np.int32), topo=np.asarray(topo, np.int32).reshape(-1, 2), levels=levels)
+
+
 def _next_pow2(v: int) -> int:
     p = 1
     while p < v:
@@ -70,10 +137,15 @@ class RayScene:
     """templates: list of [n_i,9] float32 triangle arrays (n_i <= tris_per_object; split bigger
     meshes into several templates sharing a pose).  obj_template / obj_seg_counter: int [E,K].
     obj_pose: float32 device tensor [E,K,>=7] (e.g. env_asset_state_tensor, a view is fine as long
-    as the last dim is contiguous and rows are uniformly strided)."""
+    as the last dim is contiguous and rows are uniformly strided).
+    mesh_templates: list of [n_m,9] triangle arrays of any size (URDF <mesh> / <sphere> visuals); template index
+    len(templates) + m in obj_template.  Each such object is one mesh object with its own bottom-level BVH (build_blas);
+    its face ids follow the array's order.  tmpl_seg_base / tmpl_seg_mask (and tmpl_obb, zero rows for meshes) cover
+    templates + mesh_templates."""
 
     def __init__(self, templates, tmpl_seg_base, tmpl_seg_mask, obj_template, obj_seg_counter, obj_pose: torch.Tensor,
-                 device="cuda:0", tris_per_object: Optional[int] = None, bounds_min=None, bounds_max=None, tmpl_obb=None):
+                 device="cuda:0", tris_per_object: Optional[int] = None, bounds_min=None, bounds_max=None, tmpl_obb=None,
+                 mesh_templates=None):
         """tmpl_obb: optional [T,16] oriented-box records (box_obb) of the templates that ARE boxes (valid=1);
         purely a culling aid -- results are identical with or without it."""
         self.lib = _lib.load()
@@ -83,14 +155,22 @@ class RayScene:
         dev = self.device
         obj_template = np.asarray(obj_template, dtype=np.int32)
         E, K = obj_template.shape
-        L = int(tris_per_object or max(len(t) for t in templates))
+        meshes = [np.asarray(t, np.float32).reshape(-1, 9) for t in (mesh_templates or [])]
+        nT, M = len(templates), len(meshes)
+        L = int(tris_per_object or max([len(t) for t in templates] or [1]))
         if any(len(t) > L for t in templates):
             raise ValueError("template larger than tris_per_object: split it on the host")
-        offs = np.zeros(len(templates) + 1, dtype=np.int32)
-        offs[1:] = np.cumsum([len(t) for t in templates])
-        tris = np.concatenate([np.asarray(t, np.float32).reshape(-1, 9) for t in templates], axis=0)
-        seg_base = np.concatenate([np.broadcast_to(np.asarray(b, np.int32), (len(t),)) for b, t in zip(tmpl_seg_base, templates)])
-        seg_mask = np.concatenate([np.broadcast_to(np.asarray(m, np.int32), (len(t),)) for m, t in zip(tmpl_seg_mask, templates)])
+        if len(tmpl_seg_base) != nT + M or len(tmpl_seg_mask) != nT + M:
+            raise ValueError("tmpl_seg_base / tmpl_seg_mask need one entry per template and mesh template")
+        if obj_template.min() < 0 or obj_template.max() >= nT + M:
+            raise ValueError("obj_template out of range")
+        offs = np.zeros(nT + M + 1, dtype=np.int32)  # mesh templates have no cluster triangles
+        offs[1:nT + 1] = np.cumsum([len(t) for t in templates])
+        offs[nT + 1:] = offs[nT]
+        pad = [] if offs[nT] else [np.zeros(1, np.int32)]  # a scene of mesh objects only: keep the cluster tables non-empty
+        tris = np.concatenate([np.asarray(t, np.float32).reshape(-1, 9) for t in templates] + [np.zeros((len(pad), 9), np.float32)], axis=0)
+        seg_base = np.concatenate([np.broadcast_to(np.asarray(b, np.int32), (len(t),)) for b, t in zip(tmpl_seg_base, templates)] + pad)
+        seg_mask = np.concatenate([np.broadcast_to(np.asarray(m, np.int32), (len(t),)) for m, t in zip(tmpl_seg_mask, templates)] + pad)
         T = lambda a, dt: torch.tensor(np.ascontiguousarray(a), dtype=dt, device=dev)
         self.E, self.K, self.L, self.P = E, K, L, _next_pow2(K)
         self.tmpl_tri_offset = T(offs, torch.int32)
@@ -112,12 +192,12 @@ class RayScene:
         self.face_offset = torch.zeros(E * K, dtype=torch.int32, device=dev)
         self.tmpl_obb = self.obb = None
         if tmpl_obb is not None:
-            tmpl_obb = np.asarray(tmpl_obb, dtype=np.float32).reshape(len(templates), 16)
+            tmpl_obb = np.asarray(tmpl_obb, dtype=np.float32).reshape(nT + M, 16)
             self.tmpl_obb = T(tmpl_obb, torch.float32)
             self.obb = torch.zeros(E * K * 16, dtype=torch.float32, device=dev)
         s = AgxHp2Scene()
         s.num_envs, s.num_objects, s.leaves_pow2, s.tris_per_object = E, K, self.P, L
-        s.num_templates, s.obj_pose_stride = len(templates), obj_pose.stride(1)
+        s.num_templates, s.obj_pose_stride = nT + M, obj_pose.stride(1)
         for name in ("tmpl_tri_offset", "tmpl_tris", "tmpl_seg_base", "tmpl_seg_mask", "obj_pose", "obj_template",
                      "obj_seg_counter", "tris", "nodes", "leaf_object", "face_offset"):
             setattr(s, name, getattr(self, name).data_ptr())
@@ -125,7 +205,43 @@ class RayScene:
         s.obb = self.obb.data_ptr() if self.obb is not None else None
         s.bounds_min = bounds_min.data_ptr() if bounds_min is not None else None
         s.bounds_max = bounds_max.data_ptr() if bounds_max is not None else None
+        if M:
+            self._set_meshes(s, meshes, tmpl_seg_base[nT:], tmpl_seg_mask[nT:], obj_template, nT)
         self.c = s
+
+    def _set_meshes(self, s, meshes, seg_base, seg_mask, obj_template, T):
+        """device tables of the mesh templates (one BLAS each) and the per-env mesh slabs"""
+        dev, M, (E, K) = self.device, len(meshes), obj_template.shape
+        T_ = lambda a, dt: torch.tensor(np.ascontiguousarray(a), dtype=dt, device=dev)
+        blas = [build_blas(m) for m in meshes]
+        n_tri = np.array([len(m) for m in meshes], np.int64)
+        n_node = np.array([len(b["topo"]) for b in blas], np.int64)
+        mesh_of = np.full(T + M, -1, np.int32)
+        mesh_of[T:] = np.arange(M)
+        om = mesh_of[obj_template]  # [E,K]
+        is_mesh = om >= 0
+        cnt_t = np.where(is_mesh, n_tri[np.maximum(om, 0)], 0)
+        cnt_n = np.where(is_mesh, n_node[np.maximum(om, 0)], 0)
+        slot = np.stack([np.cumsum(cnt_t, axis=1) - cnt_t, np.cumsum(cnt_n, axis=1) - cnt_n], axis=-1)
+        slot[~is_mesh] = -1
+        per_t, per_n = max(int(cnt_t.sum(axis=1).max()), 1), max(int(cnt_n.sum(axis=1).max()), 1)
+        if per_t * E * 48 > 2 ** 40 or per_t >= 2 ** 31:
+            raise ValueError("mesh storage too large")
+        self.tmpl_mesh = T_(mesh_of, torch.int32)
+        self.mesh_tri_offset = T_(np.concatenate([[0], np.cumsum(n_tri)]), torch.int32)
+        self.mesh_tris = T_(np.concatenate([m[b["order"]] for m, b in zip(meshes, blas)]), torch.float32)
+        self.mesh_tri_index = T_(np.concatenate([b["order"] for b in blas]), torch.int32)
+        self.mesh_seg = T_(np.stack([np.asarray(seg_base, np.int32), np.asarray(seg_mask, np.int32)], axis=1), torch.int32)
+        self.mesh_node_offset = T_(np.concatenate([[0], np.cumsum(n_node)]), torch.int32)
+        self.mesh_topo = T_(np.concatenate([b["topo"] for b in blas]), torch.int32)
+        self.mesh_levels = T_(np.stack([b["levels"] for b in blas]), torch.int32)
+        self.obj_mesh_slot = T_(slot, torch.int32)
+        self.mesh_world_tris = torch.zeros(E * per_t * 12, dtype=torch.float32, device=dev)
+        self.mesh_world_nodes = torch.zeros(E * per_n * 8, dtype=torch.float32, device=dev)
+        s.num_meshes, s.mesh_tris_per_env, s.mesh_nodes_per_env = M, per_t, per_n
+        for name in ("tmpl_mesh", "mesh_tri_offset", "mesh_tris", "mesh_tri_index", "mesh_seg", "mesh_node_offset", "mesh_topo",
+                     "mesh_levels", "obj_mesh_slot", "mesh_world_tris", "mesh_world_nodes"):
+            setattr(s, name, getattr(self, name).data_ptr())
 
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)

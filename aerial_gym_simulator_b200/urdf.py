@@ -1,4 +1,4 @@
-"""Minimal URDF reader: inertials, fixed-joint tree, box visuals.
+"""Minimal URDF reader: inertials, fixed-joint tree, box / cylinder / sphere / mesh visuals.
 
 Replaces what the reference obtains from Isaac Gym asset properties
 (robots/robot_manager.py:295-435: per-body mass / COM / inertia, body poses) and from
@@ -139,7 +139,8 @@ def _parse_geometry(el, base_dir) -> Optional[Visual]:
         return Visual("cylinder", np.array([float(c.get("radius")), float(c.get("length"))]), R, p)
     m = geom.find("mesh")
     if m is not None:
-        return Visual("mesh", _vec(m.get("scale"), default=1.0), R, p, os.path.join(base_dir, m.get("filename", "")))
+        fn = m.get("filename", "")
+        return Visual("mesh", _vec(m.get("scale"), default=1.0), R, p, fn if "://" in fn else os.path.join(base_dir, fn))
     return None
 
 
@@ -204,13 +205,67 @@ def box_visual_triangles(model: UrdfModel, use_collision=False):
     return out
 
 
+def _obj_triangles(path) -> np.ndarray:
+    verts, tris = [], []
+    with open(path, "r", errors="replace") as f:
+        for line in f:
+            tok = line.split()
+            if not tok:
+                continue
+            if tok[0] == "v":
+                verts.append([float(x) for x in tok[1:4]])
+            elif tok[0] == "f":
+                # "i", "i/t", "i//n", "i/t/n"; negative indices count back from the last vertex read so far
+                idx = [int(t.split("/")[0]) for t in tok[1:]]
+                idx = [i - 1 if i > 0 else len(verts) + i for i in idx]
+                for j in range(1, len(idx) - 1):  # fan triangulation of a polygon
+                    tris.append((idx[0], idx[j], idx[j + 1]))
+    if not tris:
+        raise ValueError(f"{path}: no faces")
+    v = np.asarray(verts, dtype=np.float64)
+    return v[np.asarray(tris)].reshape(-1, 9)
+
+
+def _stl_triangles(path) -> np.ndarray:
+    with open(path, "rb") as f:
+        data = f.read()
+    if len(data) >= 84:
+        n = int(np.frombuffer(data, "<u4", 1, 80)[0])
+        if len(data) == 84 + 50 * n:  # binary: header, count, n x (normal, 3 vertices, attribute)
+            rec = np.frombuffer(data, np.dtype([("n", "<f4", 3), ("v", "<f4", 9), ("a", "<u2")]), n, 84)
+            return rec["v"].astype(np.float64)
+    if not data.lstrip().startswith(b"solid"):
+        raise ValueError(f"{path}: neither binary nor ASCII STL")
+    v = [[float(x) for x in line.split()[1:4]] for line in data.decode("ascii", "replace").splitlines() if line.split()[:1] == ["vertex"]]
+    if not v or len(v) % 3:
+        raise ValueError(f"{path}: malformed ASCII STL")
+    return np.asarray(v, dtype=np.float64).reshape(-1, 9)
+
+
+def load_mesh(path, scale=(1.0, 1.0, 1.0)) -> np.ndarray:
+    """[n,9] float64 triangles (v0,v1,v2) of a Wavefront OBJ or STL (ASCII or binary) file, in the file's face order, vertices
+    multiplied by `scale`.  Polygons are fan-triangulated.  trimesh's load-time processing (vertex merge, removal of degenerate
+    faces) is not applied, so face i here is the file's face i.  Any other format, or a URI (package://...), raises ValueError."""
+    if "://" in path:
+        raise ValueError(f"mesh {path}: URIs are not resolved; give a path relative to the URDF or an absolute one")
+    ext = os.path.splitext(path)[1].lower()
+    if ext == ".obj":
+        t = _obj_triangles(path)
+    elif ext == ".stl":
+        t = _stl_triangles(path)
+    else:
+        raise ValueError(f"mesh {path}: unsupported format (OBJ and STL are read)")
+    return (t.reshape(-1, 3) * np.broadcast_to(np.asarray(scale, np.float64), (3,))).reshape(-1, 9)
+
+
 def visual_parts(model: UrdfModel, use_collision=False, max_tris=12):
-    """Every <box> / <cylinder> visual of the model as ray-cast scene parts: [(link_name, link_index, triangles [n<=max_tris,9] in the
-    root frame, obb16)].  A box is one part (its 12 triangles + the oriented box the ray-caster uses for the entry-face shortcut,
-    kind 2); a cylinder is tessellated (hp2.cylinder_triangles) and cut into parts of <= max_tris triangles that share the cylinder's
-    bounding box (kind 1: culling only).  link_index counts the links that carry a visual, in urdfpy's link order -- the per-link
-    segmentation counter of assets/warp_asset.py:44-70.  Spheres / meshes are not carried (no shipped obstacle uses them)."""
-    from .hp2 import box_obb, box_triangles, cylinder_triangles
+    """Every visual of the model as ray-cast scene parts: [(link_name, link_index, triangles [n,9] in the root frame, obb16 or None)].
+    A box is one part (its 12 triangles + the oriented box the ray-caster uses for the entry-face shortcut, kind 2); a cylinder is
+    tessellated (hp2.cylinder_triangles) and cut into parts of <= max_tris triangles that share the cylinder's bounding box (kind 1:
+    culling only).  A <mesh> (OBJ / STL, load_mesh) or a <sphere> (hp2.icosphere_triangles) is ONE part of any size with obb None:
+    the scene makes it a mesh object (RayScene mesh_templates), its triangles in file order.  link_index counts the links that carry
+    a visual, in urdfpy's link order -- the per-link segmentation counter of assets/warp_asset.py:44-70."""
+    from .hp2 import box_obb, box_triangles, cylinder_triangles, icosphere_triangles
 
     tf = model.link_transforms()
     out, link_index = [], 0
@@ -225,11 +280,18 @@ def visual_parts(model: UrdfModel, use_collision=False, max_tris=12):
                 t = cylinder_triangles(v.size[0], v.size[1])
                 obb = box_obb((2 * v.size[0], 2 * v.size[0], v.size[1]), R @ v.R, R @ v.p + p)
                 obb[15] = 1.0
+            elif v.kind == "sphere":
+                t, obb = icosphere_triangles(v.size[0]), None
+            elif v.kind == "mesh":
+                t, obb = load_mesh(v.filename, v.size), None
             else:
                 continue
             had_visual = True
             t = t.reshape(-1, 3).astype(np.float64)
             t = (R @ (v.R @ t.T + v.p[:, None]) + p[:, None]).T.reshape(-1, 9).astype(np.float32)
+            if obb is None:
+                out.append((name, link_index, t, None))
+                continue
             for i in range(0, len(t), max_tris):
                 out.append((name, link_index, t[i:i + max_tris], obb))
         link_index += int(had_visual)

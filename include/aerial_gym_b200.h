@@ -442,7 +442,32 @@ typedef struct AgxHp2Scene {
      * (padded) world OBB the ray misses skip their 12 triangle tests.  Culling only -- results unchanged. */
     const float* tmpl_obb;      /* [T][16] centre.xyz, axis0.xyz, axis1.xyz, axis2.xyz, half.xyz, valid(0/1); or NULL */
     float* obb;                 /* [E][K][16] world-frame boxes written by agx_hp2_update_scene; NULL iff tmpl_obb is NULL */
+    /* ---- mesh objects (URDF <mesh> / <sphere> visuals); all 0 / NULL for a scene of triangle clusters only ----
+     * A template t with tmpl_mesh[t] = m >= 0 is mesh m: it has no cluster triangles (tmpl_tri_offset[t+1] == tmpl_tri_offset[t])
+     * and any number of mesh triangles under a bottom-level BVH (BLAS) built once by the host.  An object referencing it is ONE
+     * leaf of the env's top-level BVH; agx_hp2_update_scene writes its world triangles into the env's mesh slab and refits its
+     * BLAS boxes in world space (the reference's per-env wp.Mesh + refit).  A mesh triangle's face id (and tie-break index) is
+     * face_offset[obj] + its index in the mesh file, so face_offset is required.
+     * Storage per env: mesh_tris_per_env x 48 B (sum of the env's mesh triangles) + mesh_nodes_per_env x 32 B (sum of their
+     * BLAS nodes); the caller computes both sums and obj_mesh_slot from obj_template. */
+    int32_t num_meshes;         /* M mesh templates (0 = none) */
+    int32_t mesh_tris_per_env;  /* triangle slots of each env's mesh slab */
+    int32_t mesh_nodes_per_env; /* BLAS node slots of each env */
+    int32_t mesh_pad_;
+    const int32_t* tmpl_mesh;   /* [T] mesh index of each template, -1 = cluster template */
+    const int32_t* mesh_tri_offset;  /* [M+1] first triangle of each mesh in mesh_tris */
+    const float* mesh_tris;     /* [Fm,9] object-frame v0,v1,v2, in BLAS leaf order */
+    const int32_t* mesh_tri_index;   /* [Fm] index of each triangle in its mesh file (face order) */
+    const int32_t* mesh_seg;    /* [M,2] segmentation base, mask of each mesh (as tmpl_seg_base / tmpl_seg_mask) */
+    const int32_t* mesh_node_offset; /* [M+1] first node of each mesh in mesh_topo */
+    const int32_t* mesh_topo;   /* [Nm,2] per node, relative to its mesh: (first child, 0) for an internal node (children at
+                                   first, first+1), (first triangle, count > 0) for a leaf.  Breadth-first order. */
+    const int32_t* mesh_levels; /* [M][AGX_HP2_BLAS_MAX_DEPTH+1] nodes of depth d are [levels[d], levels[d+1]) */
+    const int32_t* obj_mesh_slot;    /* [E,K,2] first triangle, first node of the object in its env's mesh slabs; -1 = cluster */
+    float* mesh_world_tris;     /* [E][mesh_tris_per_env][12] (v0.xyz, seg bits | e1.xyz, file index bits | e2.xyz, 0) */
+    float* mesh_world_nodes;    /* [E][mesh_nodes_per_env][8] world BLAS boxes (lo.xyz, 0 | hi.xyz, 0), padded */
 } AgxHp2Scene;
+#define AGX_HP2_BLAS_MAX_DEPTH 24     /* node depths 0..23: bounds the traversal stack */
 
 #define AGX_SENSOR_CAMERA 0              /* warp_camera_kernels.py:125-282 */
 #define AGX_SENSOR_LIDAR 1               /* warp_lidar_kernels.py:13-86,130-194 */
