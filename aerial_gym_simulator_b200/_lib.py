@@ -134,6 +134,15 @@ class AgxHp2Noise(C.Structure):
                 ("max_range", f32), ("min_range", f32), ("far_out_of_range_value", f32), ("near_out_of_range_value", f32)]
 
 
+CONTACT_MAX = 8  # AGX_CONTACT_MAX
+
+
+class AgxContactParams(C.Structure):
+    _fields_ = [("radius", f32), ("contact_offset", f32), ("rest_offset", f32), ("dt", f32), ("mass", f32), ("inertia_inv", f32 * 9),
+                ("com", f32 * 3), ("friction", f32), ("max_depenetration_velocity", f32), ("force_threshold", f32),
+                ("iterations", C.c_int32), ("ground_plane", C.c_int32)]
+
+
 SENSOR_CAMERA, SENSOR_LIDAR, SENSOR_STEREO_CAMERA, SENSOR_NORMAL_FACEID_CAMERA, SENSOR_NORMAL_FACEID_LIDAR = 0, 1, 2, 3, 4
 
 
@@ -205,6 +214,8 @@ def load():
         "agx_host_alloc": [C.c_uint64, C.POINTER(C.c_void_p)],
         "agx_host_free": [C.c_void_p],
         "agx_hp2_collide": [C.POINTER(AgxHp2Scene), C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p],
+        "agx_hp2_contact": [C.POINTER(AgxHp2Scene), C.c_int, C.POINTER(AgxContactParams), C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                            C.c_void_p, C.c_void_p],
     }.items():
         try:
             fn = getattr(lib, name)
@@ -219,7 +230,7 @@ def load():
         raise AgxError("HP2 ABI struct size mismatch between _lib.py and libaerial_gym_b200.so")
     if lib.agx_sizeof(5) != C.sizeof(AgxNavRewardParams) or lib.agx_sizeof(6) != C.sizeof(AgxImuConfig) \
             or lib.agx_sizeof(7) != C.sizeof(AgxLidarNavRewardParams) or lib.agx_sizeof(8) != C.sizeof(AgxHp2Noise) \
-            or lib.agx_sizeof(9) != C.sizeof(AgxE2ERewardParams):
+            or lib.agx_sizeof(9) != C.sizeof(AgxE2ERewardParams) or lib.agx_sizeof(11) != C.sizeof(AgxContactParams):
         raise AgxError("aux ABI struct size mismatch between _lib.py and libaerial_gym_b200.so")
     if lib.agx_sizeof(0) != C.sizeof(AgxHp1Config) or lib.agx_sizeof(1) != C.sizeof(AgxHp1Buffers) \
             or lib.agx_sizeof(2) != C.sizeof(AgxHp1ResetDraws) or lib.agx_sizeof(10) != C.sizeof(AgxObsGatherPush):

@@ -60,6 +60,7 @@ uint64_t agx_sizeof(int which) {
         case 3: return sizeof(AgxHp2Scene);
         case 4: return sizeof(AgxHp2Sensor);
         case 8: return sizeof(AgxHp2Noise);
+        case 11: return sizeof(AgxContactParams);
 #endif
         default: return 0;
     }

@@ -1,0 +1,157 @@
+// Robot-environment contact (DESIGN.md "Contact mode"): the robot's collision sphere against the scene objects and the ground
+// plane, one velocity-level sequential-impulse solve after each physics sub-step.  This header holds the solve: a contact list in,
+// the velocity change and the total impulse out.  The contact search (BVH descent, closest point) is in hp2_raycast.cu.
+// AGX_DEV: device-only in the product (hp2_raycast.cu, compiled with -fmad=false), host+device in the CPU shadow build
+// (tests/csrc/contact_shadow.cu, -ffp-contract=off).  oracle/contact_oracle.py restates every line in numpy float32 in the same
+// operation order, so the three agree bit for bit.
+#pragma once
+#include "../../include/aerial_gym_b200.h"
+#include "agx_math.cuh"
+
+namespace agx {
+
+struct ContactPt {
+    float p[3];   // contact point, world frame
+    float n[3];   // unit normal, from the obstacle towards the sphere centre
+    float depth;  // penetration: radius - distance (negative while the sphere is inside the contact offset only)
+};
+
+// keep the AGX_CONTACT_MAX nearest contacts, ordered by (distance, id); id = object index, the ground plane has the largest id
+AGX_DEV int contact_insert(ContactPt* c, float* key, int* id, int n, const ContactPt& pt, float k, int obj) {
+    int i = n < AGX_CONTACT_MAX ? n : AGX_CONTACT_MAX - 1;
+    if (n == AGX_CONTACT_MAX && !(k < key[i] || (k == key[i] && obj < id[i]))) return n;
+    while (i > 0 && (k < key[i - 1] || (k == key[i - 1] && obj < id[i - 1]))) {
+        c[i] = c[i - 1];
+        key[i] = key[i - 1];
+        id[i] = id[i - 1];
+        --i;
+    }
+    c[i] = pt;
+    key[i] = k;
+    id[i] = obj;
+    return n < AGX_CONTACT_MAX ? n + 1 : n;
+}
+
+AGX_DEV float cdot(const float* a, const float* b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
+AGX_DEV void ccross(const float* a, const float* b, float* o) {
+    o[0] = a[1] * b[2] - a[2] * b[1];
+    o[1] = a[2] * b[0] - a[0] * b[2];
+    o[2] = a[0] * b[1] - a[1] * b[0];
+}
+AGX_DEV void cmatvec(const float* M, const float* x, float* o) {
+    for (int i = 0; i < 3; ++i) o[i] = M[3 * i] * x[0] + M[3 * i + 1] * x[1] + M[3 * i + 2] * x[2];
+}
+// impulse P at lever arm r: v += P / m, w += I_w^-1 (r x P)
+AGX_DEV void capply(const float* P, const float* r, float inv_m, const float* Iw, float* v, float* w) {
+    float rp[3], dw[3];
+    ccross(r, P, rp);
+    cmatvec(Iw, rp, dw);
+    for (int i = 0; i < 3; ++i) {
+        v[i] = v[i] + P[i] * inv_m;
+        w[i] = w[i] + dw[i];
+    }
+}
+// inverse effective mass of the body along direction d at lever arm r
+AGX_DEV float ckeff(const float* r, const float* d, float inv_m, const float* Iw) {
+    float rd[3], m[3];
+    ccross(r, d, rd);
+    cmatvec(Iw, rd, m);
+    return inv_m + cdot(rd, m);
+}
+// contact point velocity v + w x r
+AGX_DEV void cvel(const float* v, const float* w, const float* r, float* o) {
+    float wr[3];
+    ccross(w, r, wr);
+    for (int i = 0; i < 3; ++i) o[i] = v[i] + wr[i];
+}
+
+// One env: n contacts of the sphere whose centre is pos and orientation q (x, y, z, w).  v, w: world linear / angular velocity,
+// updated in place.  imp: sum of the accumulated contact impulses (world frame).
+AGX_DEV void contact_solve(const AgxContactParams& P, const float* pos, const float* q, float* v, float* w, const ContactPt* c, int n,
+                           float* imp) {
+    const float x = q[0], y = q[1], z = q[2], qw = q[3];
+    float R[9];
+    R[0] = 1.0f - 2.0f * (y * y + z * z);
+    R[1] = 2.0f * (x * y - z * qw);
+    R[2] = 2.0f * (x * z + y * qw);
+    R[3] = 2.0f * (x * y + z * qw);
+    R[4] = 1.0f - 2.0f * (x * x + z * z);
+    R[5] = 2.0f * (y * z - x * qw);
+    R[6] = 2.0f * (x * z - y * qw);
+    R[7] = 2.0f * (y * z + x * qw);
+    R[8] = 1.0f - 2.0f * (x * x + y * y);
+    float com[3], A[9], Iw[9];
+    cmatvec(R, P.com, com);
+    for (int i = 0; i < 3; ++i) com[i] = pos[i] + com[i];
+    for (int i = 0; i < 3; ++i)  // A = R I^-1, Iw = A R^T
+        for (int j = 0; j < 3; ++j) A[3 * i + j] = R[3 * i] * P.inertia_inv[j] + R[3 * i + 1] * P.inertia_inv[3 + j] + R[3 * i + 2] * P.inertia_inv[6 + j];
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) Iw[3 * i + j] = A[3 * i] * R[3 * j] + A[3 * i + 1] * R[3 * j + 1] + A[3 * i + 2] * R[3 * j + 2];
+    const float inv_m = 1.0f / P.mass;
+    float r[AGX_CONTACT_MAX][3], kn[AGX_CONTACT_MAX], bias[AGX_CONTACT_MAX], ln[AGX_CONTACT_MAX], lt[AGX_CONTACT_MAX][3];
+    for (int i = 0; i < n; ++i) {
+        for (int k = 0; k < 3; ++k) {
+            r[i][k] = c[i].p[k] - com[k];
+            lt[i][k] = 0.0f;
+        }
+        kn[i] = ckeff(r[i], c[i].n, inv_m, Iw);
+        bias[i] = fminf(fmaxf(c[i].depth - P.rest_offset, 0.0f) / P.dt, P.max_depenetration_velocity);
+        ln[i] = 0.0f;
+    }
+    for (int it = 0; it < P.iterations; ++it) {
+        for (int i = 0; i < n; ++i) {
+            const float* nn = c[i].n;
+            float vr[3], dP[3];
+            // normal: accumulated impulse >= 0, target separating velocity bias
+            cvel(v, w, r[i], vr);
+            float dl = (bias[i] - cdot(nn, vr)) / kn[i];
+            const float l1 = fmaxf(ln[i] + dl, 0.0f);
+            dl = l1 - ln[i];
+            ln[i] = l1;
+            for (int k = 0; k < 3; ++k) dP[k] = nn[k] * dl;
+            capply(dP, r[i], inv_m, Iw, v, w);
+            // friction: drive the tangential velocity to 0, accumulated impulse inside the circle mu * ln
+            cvel(v, w, r[i], vr);
+            const float vn = cdot(nn, vr);
+            float vt[3], l2[3];
+            for (int k = 0; k < 3; ++k) {
+                vt[k] = vr[k] - nn[k] * vn;
+                l2[k] = lt[i][k];
+            }
+            const float s = sqrtf(cdot(vt, vt));
+            if (s > 0.0f) {
+                float t[3];
+                for (int k = 0; k < 3; ++k) t[k] = vt[k] / s;
+                const float dt_ = s / ckeff(r[i], t, inv_m, Iw);
+                for (int k = 0; k < 3; ++k) l2[k] = l2[k] - t[k] * dt_;
+            }
+            const float mag = sqrtf(cdot(l2, l2)), lim = P.friction * ln[i];
+            if (mag > lim) {
+                const float f = lim / mag;
+                for (int k = 0; k < 3; ++k) l2[k] = l2[k] * f;
+            }
+            for (int k = 0; k < 3; ++k) {
+                dP[k] = l2[k] - lt[i][k];
+                lt[i][k] = l2[k];
+            }
+            capply(dP, r[i], inv_m, Iw, v, w);
+        }
+    }
+    imp[0] = imp[1] = imp[2] = 0.0f;
+    for (int i = 0; i < n; ++i)
+        for (int k = 0; k < 3; ++k) imp[k] = imp[k] + c[i].n[k] * ln[i] + lt[i][k];
+}
+
+// the per-env epilogue: solve, contact force = impulse / dt, crash flag when |F| exceeds the threshold (the reference's rule)
+AGX_DEV void contact_env(const AgxContactParams& P, float* rs, const ContactPt* c, int n, float* force, uint8_t* crash) {
+    float v[3] = {rs[7], rs[8], rs[9]}, w[3] = {rs[10], rs[11], rs[12]}, imp[3];
+    contact_solve(P, rs, rs + 3, v, w, c, n, imp);
+    for (int k = 0; k < 3; ++k) {
+        rs[7 + k] = v[k];
+        rs[10 + k] = w[k];
+        force[k] = imp[k] / P.dt;
+    }
+    if (sqrtf(cdot(force, force)) > P.force_threshold) *crash = 1;
+}
+
+}  // namespace agx

@@ -28,6 +28,7 @@
 
 #include "../../include/aerial_gym_b200.h"
 #include "agx_common.cuh"
+#include "contact_core.cuh"
 
 namespace {
 
@@ -922,6 +923,165 @@ hp2_collide_kernel(const __grid_constant__ AgxHp2Scene sc, const float* __restri
     if (min_dist) min_dist[e] = sqrtf(best);
 }
 
+// ---- contact mode (agx_hp2_contact): per object the closest point, then the solve of contact_core.cuh --------------------------
+// point_tri_dist2's Voronoi regions, returning the closest point itself
+__device__ __forceinline__ v3 closest_point_tri(v3 p, v3 a, v3 ab, v3 ac) {
+    v3 ap = sub3(p, a);
+    float d1 = dot3(ab, ap), d2 = dot3(ac, ap);
+    if (d1 <= 0.0f && d2 <= 0.0f) return a;
+    v3 b{a.x + ab.x, a.y + ab.y, a.z + ab.z};
+    v3 bp = sub3(p, b);
+    float d3 = dot3(ab, bp), d4 = dot3(ac, bp);
+    if (d3 >= 0.0f && d4 <= d3) return b;
+    float vc = fmaf(d1, d4, -(d3 * d2));
+    if (vc <= 0.0f && d1 >= 0.0f && d3 <= 0.0f) {
+        float v = d1 / (d1 - d3);
+        return v3{fmaf(v, ab.x, a.x), fmaf(v, ab.y, a.y), fmaf(v, ab.z, a.z)};
+    }
+    v3 c{a.x + ac.x, a.y + ac.y, a.z + ac.z};
+    v3 cp = sub3(p, c);
+    float d5 = dot3(ab, cp), d6 = dot3(ac, cp);
+    if (d6 >= 0.0f && d5 <= d6) return c;
+    float vb = fmaf(d5, d2, -(d1 * d6));
+    if (vb <= 0.0f && d2 >= 0.0f && d6 <= 0.0f) {
+        float w = d2 / (d2 - d6);
+        return v3{fmaf(w, ac.x, a.x), fmaf(w, ac.y, a.y), fmaf(w, ac.z, a.z)};
+    }
+    float va = fmaf(d3, d6, -(d5 * d4));
+    if (va <= 0.0f && (d4 - d3) >= 0.0f && (d5 - d6) >= 0.0f) {
+        float w = (d4 - d3) / ((d4 - d3) + (d5 - d6));
+        v3 bc = sub3(c, b);
+        return v3{fmaf(w, bc.x, b.x), fmaf(w, bc.y, b.y), fmaf(w, bc.z, b.z)};
+    }
+    float denom = 1.0f / (va + vb + vc);
+    float v = vb * denom, w = vc * denom;
+    return v3{fmaf(w, ac.x, fmaf(v, ab.x, a.x)), fmaf(w, ac.y, fmaf(v, ab.y, a.y)), fmaf(w, ac.z, fmaf(v, ab.z, a.z))};
+}
+
+// the closest triangle of one object: squared distance, closest point, the triangle's slab (its face normal when d2 == 0)
+struct ObjClosest {
+    float d2;
+    v3 q;
+    const float4* tri;
+};
+__device__ __forceinline__ void tri_closest(v3 c, const float4* tp, ObjClosest& best) {
+    const float4 a = tp[0], b = tp[1], cc = tp[2];
+    const v3 q = closest_point_tri(c, v3{a.x, a.y, a.z}, v3{b.x, b.y, b.z}, v3{cc.x, cc.y, cc.z});
+    const v3 d = sub3(c, q);
+    const float d2 = dot3(d, d);
+    if (d2 < best.d2) best = ObjClosest{d2, q, tp};
+}
+
+// one mesh object: the BLAS descent of mesh_sphere_min, keeping the closest point
+__device__ __noinline__ void mesh_closest(const AgxHp2Scene& sc, const MeshCtx& mc, int obj, v3 c, float search, ObjClosest& best) {
+    const int m = sc.tmpl_mesh[mc.obj_template[obj]];
+    const int2* topo = reinterpret_cast<const int2*>(sc.mesh_topo) + sc.mesh_node_offset[m];
+    const float* nodes = mc.nodes + (size_t)mc.slot[2 * obj + 1] * kNodeFloats;
+    const float4* tp = reinterpret_cast<const float4*>(mc.tris + (size_t)mc.slot[2 * obj] * kTriFloats);
+    int stack[AGX_HP2_BLAS_MAX_DEPTH];
+    int sp = 0, node = 0;
+    while (true) {
+        const float* nd = nodes + (size_t)node * kNodeFloats;
+        float dx = fmaxf(fmaxf(nd[0] - c.x, c.x - nd[4]), 0.0f);
+        float dy = fmaxf(fmaxf(nd[1] - c.y, c.y - nd[5]), 0.0f);
+        float dz = fmaxf(fmaxf(nd[2] - c.z, c.z - nd[6]), 0.0f);
+        float box_d2 = dx * dx + dy * dy + dz * dz;
+        if (box_d2 <= fminf(best.d2, search) * 1.0001f + 1e-6f) {  // culling only
+            const int2 t = topo[node];
+            if (t.y > 0) {
+                for (int s = t.x; s < t.x + t.y; ++s) tri_closest(c, tp + 3 * s, best);
+            } else {
+                stack[sp++] = t.x + 1;
+                node = t.x;
+                continue;
+            }
+        }
+        if (sp == 0) break;
+        node = stack[--sp];
+    }
+}
+
+// one thread per env: every object within reach (radius + contact_offset) gives its closest point, the ground plane one more;
+// the AGX_CONTACT_MAX nearest go to the solve.  sc.num_objects == 0: no scene.
+__global__ void __launch_bounds__(128)
+hp2_contact_kernel(const __grid_constant__ AgxHp2Scene sc, const __grid_constant__ AgxContactParams P, int num_envs,
+                   float* __restrict__ root_state, int stride, float* __restrict__ force, uint8_t* __restrict__ crashes,
+                   int32_t* __restrict__ contact_obj) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= num_envs) return;
+    float* rs = root_state + (size_t)e * stride;
+    const v3 c{rs[0], rs[1], rs[2]};
+    const float reach = P.radius + P.contact_offset;
+    const float search = reach * reach;
+    agx::ContactPt cp[AGX_CONTACT_MAX];
+    float key[AGX_CONTACT_MAX];
+    int id[AGX_CONTACT_MAX];
+    int n = 0;
+    const int K = sc.num_objects;
+    if (K > 0) {
+        const int P2 = sc.leaves_pow2, L = sc.tris_per_object;
+        const float* nodes = sc.nodes + (size_t)e * (2 * P2 - 1) * kNodeFloats;
+        const int32_t* leaf = sc.leaf_object + (size_t)e * (P2 < 4 ? 4 : P2);
+        const float* tris = sc.tris + (size_t)e * K * L * kTriFloats;
+        int stack[24];
+        int sp = 0, node = 0;
+        while (true) {
+            const float* nd = nodes + (size_t)node * kNodeFloats;
+            float dx = fmaxf(fmaxf(nd[0] - c.x, c.x - nd[4]), 0.0f);
+            float dy = fmaxf(fmaxf(nd[1] - c.y, c.y - nd[5]), 0.0f);
+            float dz = fmaxf(fmaxf(nd[2] - c.z, c.z - nd[6]), 0.0f);
+            float box_d2 = dx * dx + dy * dy + dz * dz;
+            if (box_d2 <= search * 1.0001f + 1e-6f) {  // padded boxes + slack: culling only
+                if (node >= P2 - 1) {
+                    const int obj = leaf[node - (P2 - 1)];
+                    ObjClosest best{3.0e38f, v3{0.0f, 0.0f, 0.0f}, nullptr};
+                    if (obj >= 0 && sc.num_meshes && sc.obj_mesh_slot[((size_t)e * K + obj) * 2] >= 0) {
+                        mesh_closest(sc, mesh_ctx(sc, e), obj, c, search, best);
+                    } else if (obj >= 0) {
+                        const float4* tp = reinterpret_cast<const float4*>(tris + (size_t)obj * L * kTriFloats);
+                        for (int s = 0; s < L; ++s) {
+                            const float4 b = tp[3 * s + 1], cc = tp[3 * s + 2];
+                            if (b.x == 0.f && b.y == 0.f && b.z == 0.f && cc.x == 0.f && cc.y == 0.f && cc.z == 0.f) continue;  // padding
+                            tri_closest(c, tp + 3 * s, best);
+                        }
+                    }
+                    if (best.d2 <= search) {
+                        const float dist = sqrtf(best.d2);
+                        v3 nv;
+                        if (dist > 0.0f) {
+                            const v3 d = sub3(c, best.q);
+                            nv = v3{d.x / dist, d.y / dist, d.z / dist};
+                        } else {  // the centre lies on the surface: the triangle's face normal
+                            const float4 b = best.tri[1], cc = best.tri[2];
+                            nv = normalize3(cross3(v3{b.x, b.y, b.z}, v3{cc.x, cc.y, cc.z}));
+                        }
+                        const agx::ContactPt pt{{best.q.x, best.q.y, best.q.z}, {nv.x, nv.y, nv.z}, P.radius - dist};
+                        n = agx::contact_insert(cp, key, id, n, pt, dist, obj);
+                    }
+                } else {
+                    stack[sp++] = 2 * node + 2;
+                    node = 2 * node + 1;
+                    continue;
+                }
+            }
+            if (sp == 0) break;
+            node = stack[--sp];
+        }
+    }
+    if (P.ground_plane && c.z <= reach) {
+        const agx::ContactPt pt{{c.x, c.y, 0.0f}, {0.0f, 0.0f, 1.0f}, P.radius - c.z};
+        n = agx::contact_insert(cp, key, id, n, pt, c.z, K);
+    }
+    if (contact_obj)
+        for (int i = 0; i < AGX_CONTACT_MAX; ++i) contact_obj[(size_t)e * AGX_CONTACT_MAX + i] = i < n ? id[i] : -1;
+    float* f = force + (size_t)e * 3;
+    if (n == 0) {
+        f[0] = f[1] = f[2] = 0.0f;
+        return;
+    }
+    agx::contact_env(P, rs, cp, n, f, crashes + e);
+}
+
 __device__ __forceinline__ float range_epilogue(const AgxHp2Sensor& s, float px) {
     // warp_sensor.py:216-225: two sequential masked assignments, then the division
     if (px > s.max_range) px = s.far_out_of_range_value;
@@ -1261,6 +1421,27 @@ int agx_hp2_collide(const AgxHp2Scene* sc, const float* robot_pose, int robot_po
     hp2_collide_kernel<<<(sc->num_envs + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*sc, robot_pose, robot_pose_stride, radius, crashes,
                                                                                   min_dist);
     return agx_check_launch("hp2_collide_kernel");
+}
+
+int agx_hp2_contact(const AgxHp2Scene* sc, int num_envs, const AgxContactParams* p, float* root_state, int root_state_stride,
+                    float* contact_force, uint8_t* crashes, int32_t* contact_obj, void* stream) {
+    AgxHp2Scene none = {};
+    if (sc) {
+        int rc = validate_scene(sc);
+        if (rc) return rc;
+        if (sc->num_envs != num_envs) return agx_set_error(AGX_E_INVALID, "num_envs %d != scene num_envs %d", num_envs, sc->num_envs);
+    }
+    if (!p) return agx_set_error(AGX_E_NULL, "params is NULL");
+    if (num_envs < 0) return agx_set_error(AGX_E_INVALID, "num_envs < 0");
+    if (!(p->radius >= 0.0f) || !(p->contact_offset >= 0.0f) || !(p->dt > 0.0f) || !(p->mass > 0.0f) || !(p->friction >= 0.0f) ||
+        !(p->max_depenetration_velocity >= 0.0f) || p->iterations < 0)
+        return agx_set_error(AGX_E_INVALID, "contact params out of range");
+    if (num_envs == 0) return AGX_OK;
+    if (!root_state || !contact_force || !crashes) return agx_set_error(AGX_E_NULL, "root_state/contact_force/crashes is NULL");
+    if (root_state_stride < 13) return agx_set_error(AGX_E_INVALID, "root_state_stride < 13");
+    hp2_contact_kernel<<<(num_envs + 127) / 128, 128, 0, (cudaStream_t)stream>>>(sc ? *sc : none, *p, num_envs, root_state,
+                                                                                  root_state_stride, contact_force, crashes, contact_obj);
+    return agx_check_launch("hp2_contact_kernel");
 }
 
 int agx_hp2_cast(const AgxHp2Scene* sc, const AgxHp2Sensor* sn, void* stream) {

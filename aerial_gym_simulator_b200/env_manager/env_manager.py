@@ -7,8 +7,14 @@ Differences that are deliberate and documented (DESIGN.md):
     view of ``vec_root_tensor``); obstacles live in ``env_asset_state_tensor`` [N,K,13];
   * construction is array-native (no O(N) actor loop), except asset-file selection which keeps the
     reference's per-env ``random.choices`` / ``random.shuffle`` order;
-  * collision flags (a14) come from a geometric sphere-vs-mesh overlap test, not PhysX contact
-    forces; ``robot_contact_force_tensor`` stays 0.
+  * contact, args['contact']:
+      - "flag" (default): collision flags (a14) come from a geometric sphere-vs-mesh overlap test, not PhysX contact forces.
+        Nothing stops the robot: with reset_on_collision = False it flies through obstacles and the ground.
+        ``robot_contact_force_tensor`` stays 0 and ``create_ground_plane`` is not read.
+      - "rigid": after every physics sub-step one velocity-level contact solve (agx_hp2_contact) stops the robot's collision
+        sphere at the obstacles and, with ``create_ground_plane``, at the plane z = 0.  It fills ``robot_contact_force_tensor``,
+        flags crashes by the reference's rule |F| > collision_force_threshold and adds the force to the IMU's force input.
+        args['contact_friction'] is the Coulomb coefficient (default 1.0).  DESIGN.md "Contact mode" has the model.
 """
 from __future__ import annotations
 
@@ -26,6 +32,7 @@ from .. import robots  # noqa: F401  (registers robots + controllers)
 from .. import urdf
 from ..hp1 import Hp1Engine
 from ..hp2 import RayScene, RaySensor
+from ..hp2 import contact as hp2_contact
 from ..registry._core import env_config_registry, robot_registry, sim_config_registry
 
 
@@ -97,6 +104,13 @@ class EnvManager:
         self.reset_rng = self.env_args.get("reset_rng", "device")
         if self.reset_rng not in ("device", "torch"):
             raise ValueError("args['reset_rng'] must be 'device' or 'torch'")
+        self.contact_mode = self.env_args.get("contact", "flag")
+        if self.contact_mode not in ("flag", "rigid"):
+            raise ValueError("args['contact'] must be 'flag' or 'rigid'")
+        mu = self.env_args.get("contact_friction", 1.0)
+        if isinstance(mu, bool) or not isinstance(mu, (int, float)) or not math.isfinite(mu) or mu < 0:
+            raise ValueError("args['contact_friction'] must be a finite number >= 0")
+        self.contact_friction = float(mu)
         self.global_tensor_dict = {}
         self.step_counter = 0
         self._graphs, self._dist_ctr_dev = {}, None
@@ -162,9 +176,19 @@ class EnvManager:
         eng.bounds_max.copy_(_lerp(self._bounds_rng[2], self._bounds_rng[3], torch.rand(N, 3, device=dev)))
         self._build_obstacles()
         self._build_sensors()
-        if eng.host_io and (self.scene is not None or self.reset_rng != "device"):
-            raise NotImplementedError("args['host_io'] needs an obstacle-free env and reset_rng='device': the flags "
+        if eng.host_io and (self.scene is not None or self.reset_rng != "device" or self.contact_mode == "rigid"):
+            raise NotImplementedError("args['host_io'] needs an obstacle-free env, reset_rng='device' and contact='flag': the flags "
                                       "live in host memory and are written only by the fused task step")
+        self.contact_params = None
+        if self.contact_mode == "rigid":
+            px, c = self.sim_config.sim.physx, eng.cfg
+            p = self.contact_params = _lib.AgxContactParams()
+            p.radius, p.contact_offset, p.rest_offset = float(self.robot.collision_radius), float(px.contact_offset), float(px.rest_offset)
+            p.dt, p.mass = float(self.sim_config.sim.dt), float(c.mass)
+            p.inertia_inv[:], p.com[:] = list(c.inertia_inv), list(c.com)
+            p.friction, p.max_depenetration_velocity = self.contact_friction, float(px.max_depenetration_velocity)
+            p.force_threshold = float(self.cfg.env.collision_force_threshold)
+            p.iterations, p.ground_plane = int(px.num_position_iterations), int(bool(getattr(self.cfg.env, "create_ground_plane", False)))
 
     # ---- obstacles: AssetLoader.select_assets_for_sim + WarpEnv (asset_loader.py:148-194, warp_env_manager.py)
     def _select_assets(self):
@@ -501,8 +525,11 @@ class EnvManager:
         with torch.cuda.stream(side):  # warm-up outside the capture (first launches may load modules), on throw-away copies of the state
             keep = (eng.root_state.clone(), eng.motor_thrust.clone(), self.collision_tensor.clone(),
                     None if not dist else self._dist_ctr_dev.clone())
+            force = self.global_tensor_dict["robot_contact_force_tensor"]
+            keep_force = force.clone()
             body()
             eng.root_state.copy_(keep[0]); eng.motor_thrust.copy_(keep[1]); self.collision_tensor.copy_(keep[2])
+            force.copy_(keep_force)
             if dist:
                 self._dist_ctr_dev.copy_(keep[3])
         cur.wait_stream(side)
@@ -533,8 +560,9 @@ class EnvManager:
         gtd["robot_prev_actions"][:] = gtd["robot_actions"]  # robot_manager.py:486-488
         gtd["robot_actions"][:] = actions
         a = gtd["robot_actions"]
-        if self.spec.enable_disturbance or self.scene is not None:
-            # the reference loop (env_manager.py:426-428): fresh disturbance draws and a collision check after EVERY physics step
+        if self.spec.enable_disturbance or self.scene is not None or self.contact_params is not None:
+            # the reference loop (env_manager.py:426-428): fresh disturbance draws and a collision check (or contact solve) after
+            # EVERY physics step
             if self.step_mode == "graph":
                 self._graph_for(n).replay()  # the n x (physics launch with in-kernel draw, collision launch) of this env step: one graph launch
                 if self.spec.enable_disturbance:
@@ -589,8 +617,12 @@ class EnvManager:
 
     def compute_observations(self):
         """crashes += contact (env_manager.py:358-362).  PhysX contact forces are replaced by a
-        geometric test: the base-link collision sphere overlaps the env mesh (agx_hp2_collide)."""
-        if self.scene is not None:
+        geometric test: the base-link collision sphere overlaps the env mesh (agx_hp2_collide).  Contact mode: the contact solve
+        (agx_hp2_contact) in its place, which flags by the contact force as the reference does."""
+        if self.contact_params is not None:
+            hp2_contact(self.scene, self.engine.root_state, self.contact_params, self.global_tensor_dict["robot_contact_force_tensor"],
+                        self.collision_tensor)
+        elif self.scene is not None:
             self.scene.collide(self.engine.root_state, self.robot.collision_radius, self.collision_tensor)
 
     def reset_terminated_and_truncated_envs(self):
@@ -609,6 +641,8 @@ class EnvManager:
             gtd = self.global_tensor_dict
             fs, w = gtd["force_sensor_tensor"], self.engine.body_wrench
             fs[:, 0:3] = w[:, 0:3] + gtd["robot_mass"].unsqueeze(1) * _quat_rotate_inverse(gtd["robot_orientation"], gtd["gravity"])
+            if self.contact_params is not None:  # PhysX's force sensor includes the contact force
+                fs[:, 0:3] += _quat_rotate_inverse(gtd["robot_orientation"], gtd["robot_contact_force_tensor"])
             fs[:, 3:6] = w[:, 3:6]
             self.imu.update()
         if self.sensor is None:

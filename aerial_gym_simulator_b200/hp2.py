@@ -265,6 +265,39 @@ class RayScene:
                                             C.c_float(radius), C.c_void_p(crashes.data_ptr()), md, self._stream()),
                    "agx_hp2_collide")
 
+    def contact(self, robot_state: torch.Tensor, params: _lib.AgxContactParams, force: torch.Tensor, crashes: torch.Tensor,
+                contact_obj: Optional[torch.Tensor] = None):
+        """One rigid-contact solve against this scene (and the ground plane if params.ground_plane): see contact()."""
+        contact(self, robot_state, params, force, crashes, contact_obj)
+
+
+def contact(scene: Optional[RayScene], robot_state: torch.Tensor, params: _lib.AgxContactParams, force: torch.Tensor,
+            crashes: torch.Tensor, contact_obj: Optional[torch.Tensor] = None):
+    """agx_hp2_contact: the robot's collision sphere against the scene's objects (scene None: none) and the ground plane.
+    robot_state [E,>=13] float32: linear and world angular velocity updated in place; force [E,3] float32 = contact impulse / dt;
+    crashes (bool [E]) |= |force| > params.force_threshold; contact_obj (int32 [E,CONTACT_MAX], optional) = contacts used."""
+    E = robot_state.shape[0]
+    dev = robot_state.device
+    if dev.type != "cuda":
+        raise _lib.AgxError("contact needs a CUDA device: there is no CPU path")
+    if scene is not None and (scene.E != E or scene.device != dev):
+        raise ValueError("robot_state must have one row per scene env, on the scene's device")
+    if robot_state.dtype != torch.float32 or robot_state.dim() != 2 or robot_state.shape[1] < 13 or robot_state.stride(1) != 1:
+        raise ValueError("robot_state must be float32 [E,>=13] with contiguous rows")
+    if crashes.dtype != torch.bool or crashes.shape != (E,) or crashes.device != dev:
+        raise ValueError("crashes must be bool [E]")
+    if force.dtype != torch.float32 or force.shape != (E, 3) or not force.is_contiguous() or force.device != dev:
+        raise ValueError("force must be contiguous float32 [E,3]")
+    if contact_obj is not None and (contact_obj.dtype != torch.int32 or contact_obj.shape != (E, _lib.CONTACT_MAX)
+                                    or not contact_obj.is_contiguous() or contact_obj.device != dev):
+        raise ValueError(f"contact_obj must be contiguous int32 [E,{_lib.CONTACT_MAX}]")
+    lib = _lib.load()
+    co = C.c_void_p(contact_obj.data_ptr()) if contact_obj is not None else None
+    _lib.check(lib.agx_hp2_contact(C.byref(scene.c) if scene is not None else None, E, C.byref(params),
+                                   C.c_void_p(robot_state.data_ptr()), robot_state.stride(0), C.c_void_p(force.data_ptr()),
+                                   C.c_void_p(crashes.data_ptr()), co, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+               "agx_hp2_contact")
+
 
 def camera_intrinsics(width, height, horizontal_fov_deg):
     """WarpCam.initialize_camera_matrices (sensors/warp/warp_cam.py:31-64): fp32 K, its inverse."""

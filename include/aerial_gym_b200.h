@@ -172,7 +172,8 @@ int agx_abi_version(void);
 const char* agx_last_error(void);
 /* sizeof() of the ABI structs as compiled into the library (binding self-check):
  * which = 0 AgxHp1Config, 1 AgxHp1Buffers, 2 AgxHp1ResetDraws, 3 AgxHp2Scene, 4 AgxHp2Sensor,
- * 5 AgxNavRewardParams, 6 AgxImuConfig, 7 AgxLidarNavRewardParams, 8 AgxHp2Noise, 9 AgxE2ERewardParams, 10 AgxObsGatherPush */
+ * 5 AgxNavRewardParams, 6 AgxImuConfig, 7 AgxLidarNavRewardParams, 8 AgxHp2Noise, 9 AgxE2ERewardParams, 10 AgxObsGatherPush,
+ * 11 AgxContactParams */
 uint64_t agx_sizeof(int which);
 
 /* Host buffers the kernels can address directly (pinned, portable, mapped: cudaHostAlloc).
@@ -519,6 +520,38 @@ int agx_hp2_cast(const AgxHp2Scene* scene, const AgxHp2Sensor* sensor, void* str
  *   min_dist [E] f32  : distance from the sphere centre to the closest triangle, or NULL */
 int agx_hp2_collide(const AgxHp2Scene* scene, const float* robot_pose, int robot_pose_stride, float radius,
                     uint8_t* crashes, float* min_dist, void* stream);
+
+/* Rigid contact (opt-in replacement of the geometric flag above; DESIGN.md "Contact mode").  The robot is its collision sphere
+ * (centre = root_state[0:3], `radius`).  Contacts: each scene object whose closest triangle is within radius + contact_offset
+ * (point = closest point on that triangle, normal = from it to the centre, or the face normal when the centre lies on it), and,
+ * with ground_plane, the plane z = 0 (normal +z); the AGX_CONTACT_MAX nearest are kept, ties to the lower object index, the
+ * ground last.  One sequential-impulse solve (`iterations` passes; per contact a normal impulse >= 0 with target separating
+ * velocity min(max(depth - rest_offset, 0) / dt, max_depenetration_velocity), then Coulomb friction with a circular clamp
+ * |lambda_t| <= friction * lambda_n).  Obstacles are kinematic and at rest.  Lever arms are taken about p + R com. */
+#define AGX_CONTACT_MAX 8
+typedef struct AgxContactParams {
+    float radius;               /* robot collision sphere */
+    float contact_offset;       /* contacts are generated within radius + contact_offset */
+    float rest_offset;          /* penetration the solve leaves in place */
+    float dt;                   /* physics sub-step */
+    float mass;
+    float inertia_inv[9];       /* body frame, row-major */
+    float com[3];               /* centre of mass, body frame */
+    float friction;             /* Coulomb coefficient */
+    float max_depenetration_velocity;
+    float force_threshold;      /* crashes |= |contact force| > force_threshold */
+    int32_t iterations;
+    int32_t ground_plane;       /* 1: the plane z = 0 is solid */
+} AgxContactParams;
+
+/* One solve per env after a physics sub-step.  scene may be NULL (no objects: a ground-only env).
+ *   root_state    [E,stride] : linear (7:10) and world angular (10:13) velocity updated in place; pose read only
+ *   contact_force [E,3] f32  : sum of the contact impulses / dt, world frame (0 without contact)
+ *   crashes       [E] bool   : OR-ed with |contact_force| > force_threshold
+ *   contact_obj   [E,AGX_CONTACT_MAX] int32 or NULL : the contacts used, nearest first (object index, num_objects = the ground,
+ *                             -1 = unused slot) */
+int agx_hp2_contact(const AgxHp2Scene* scene, int num_envs, const AgxContactParams* params, float* root_state, int root_state_stride,
+                    float* contact_force, uint8_t* crashes, int32_t* contact_obj, void* stream);
 
 
 /* ======================================================================================
