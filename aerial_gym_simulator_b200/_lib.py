@@ -143,6 +143,10 @@ class AgxContactParams(C.Structure):
                 ("iterations", C.c_int32), ("ground_plane", C.c_int32)]
 
 
+class AgxContactMotion(C.Structure):
+    _fields_ = [("asset_state", C.c_void_p), ("asset_stride", C.c_int32), ("num_assets", C.c_int32), ("obj_asset", C.c_void_p)]
+
+
 SENSOR_CAMERA, SENSOR_LIDAR, SENSOR_STEREO_CAMERA, SENSOR_NORMAL_FACEID_CAMERA, SENSOR_NORMAL_FACEID_LIDAR = 0, 1, 2, 3, 4
 
 
@@ -216,6 +220,8 @@ def load():
         "agx_hp2_collide": [C.POINTER(AgxHp2Scene), C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p],
         "agx_hp2_contact": [C.POINTER(AgxHp2Scene), C.c_int, C.POINTER(AgxContactParams), C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                             C.c_void_p, C.c_void_p],
+        "agx_hp2_contact_moving": [C.POINTER(AgxHp2Scene), C.c_int, C.POINTER(AgxContactParams), C.POINTER(AgxContactMotion), C.c_void_p,
+                                   C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
     }.items():
         try:
             fn = getattr(lib, name)
@@ -230,7 +236,8 @@ def load():
         raise AgxError("HP2 ABI struct size mismatch between _lib.py and libaerial_gym_b200.so")
     if lib.agx_sizeof(5) != C.sizeof(AgxNavRewardParams) or lib.agx_sizeof(6) != C.sizeof(AgxImuConfig) \
             or lib.agx_sizeof(7) != C.sizeof(AgxLidarNavRewardParams) or lib.agx_sizeof(8) != C.sizeof(AgxHp2Noise) \
-            or lib.agx_sizeof(9) != C.sizeof(AgxE2ERewardParams) or lib.agx_sizeof(11) != C.sizeof(AgxContactParams):
+            or lib.agx_sizeof(9) != C.sizeof(AgxE2ERewardParams) or lib.agx_sizeof(11) != C.sizeof(AgxContactParams) \
+            or lib.agx_sizeof(12) != C.sizeof(AgxContactMotion):
         raise AgxError("aux ABI struct size mismatch between _lib.py and libaerial_gym_b200.so")
     if lib.agx_sizeof(0) != C.sizeof(AgxHp1Config) or lib.agx_sizeof(1) != C.sizeof(AgxHp1Buffers) \
             or lib.agx_sizeof(2) != C.sizeof(AgxHp1ResetDraws) or lib.agx_sizeof(10) != C.sizeof(AgxObsGatherPush):

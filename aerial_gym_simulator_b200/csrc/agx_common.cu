@@ -61,6 +61,7 @@ uint64_t agx_sizeof(int which) {
         case 4: return sizeof(AgxHp2Sensor);
         case 8: return sizeof(AgxHp2Noise);
         case 11: return sizeof(AgxContactParams);
+        case 12: return sizeof(AgxContactMotion);
 #endif
         default: return 0;
     }

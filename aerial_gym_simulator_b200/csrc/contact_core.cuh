@@ -64,11 +64,20 @@ AGX_DEV void cvel(const float* v, const float* w, const float* r, float* o) {
     ccross(w, r, wr);
     for (int i = 0; i < 3; ++i) o[i] = v[i] + wr[i];
 }
+// velocity of a moving obstacle at the contact point p: its asset row (x y z qx qy qz qw vx vy vz wx wy wz) gives v + w x (p - x)
+AGX_DEV void obstacle_point_vel(const float* row, const float* p, float* u) {
+    const float r[3] = {p[0] - row[0], p[1] - row[1], p[2] - row[2]};
+    cvel(row + 7, row + 10, r, u);
+}
 
 // One env: n contacts of the sphere whose centre is pos and orientation q (x, y, z, w).  v, w: world linear / angular velocity,
 // updated in place.  imp: sum of the accumulated contact impulses (world frame).
+// MOVING (agx_hp2_contact_moving): u[i] is the velocity of contact i's obstacle at its contact point, and both rows act on the
+// relative velocity v_robot(p) - u.  The obstacle is kinematic (infinite mass), so only the robot's velocity changes.  Without
+// MOVING no u is read and the code is the static solve's.
+template <bool MOVING = false>
 AGX_DEV void contact_solve(const AgxContactParams& P, const float* pos, const float* q, float* v, float* w, const ContactPt* c, int n,
-                           float* imp) {
+                           float* imp, const float (*u)[3] = nullptr) {
     const float x = q[0], y = q[1], z = q[2], qw = q[3];
     float R[9];
     R[0] = 1.0f - 2.0f * (y * y + z * z);
@@ -104,6 +113,8 @@ AGX_DEV void contact_solve(const AgxContactParams& P, const float* pos, const fl
             float vr[3], dP[3];
             // normal: accumulated impulse >= 0, target separating velocity bias
             cvel(v, w, r[i], vr);
+            if (MOVING)
+                for (int k = 0; k < 3; ++k) vr[k] = vr[k] - u[i][k];
             float dl = (bias[i] - cdot(nn, vr)) / kn[i];
             const float l1 = fmaxf(ln[i] + dl, 0.0f);
             dl = l1 - ln[i];
@@ -112,6 +123,8 @@ AGX_DEV void contact_solve(const AgxContactParams& P, const float* pos, const fl
             capply(dP, r[i], inv_m, Iw, v, w);
             // friction: drive the tangential velocity to 0, accumulated impulse inside the circle mu * ln
             cvel(v, w, r[i], vr);
+            if (MOVING)
+                for (int k = 0; k < 3; ++k) vr[k] = vr[k] - u[i][k];
             const float vn = cdot(nn, vr);
             float vt[3], l2[3];
             for (int k = 0; k < 3; ++k) {
@@ -143,9 +156,11 @@ AGX_DEV void contact_solve(const AgxContactParams& P, const float* pos, const fl
 }
 
 // the per-env epilogue: solve, contact force = impulse / dt, crash flag when |F| exceeds the threshold (the reference's rule)
-AGX_DEV void contact_env(const AgxContactParams& P, float* rs, const ContactPt* c, int n, float* force, uint8_t* crash) {
+template <bool MOVING = false>
+AGX_DEV void contact_env(const AgxContactParams& P, float* rs, const ContactPt* c, int n, float* force, uint8_t* crash,
+                         const float (*u)[3] = nullptr) {
     float v[3] = {rs[7], rs[8], rs[9]}, w[3] = {rs[10], rs[11], rs[12]}, imp[3];
-    contact_solve(P, rs, rs + 3, v, w, c, n, imp);
+    contact_solve<MOVING>(P, rs, rs + 3, v, w, c, n, imp, u);
     for (int k = 0; k < 3; ++k) {
         rs[7 + k] = v[k];
         rs[10 + k] = w[k];

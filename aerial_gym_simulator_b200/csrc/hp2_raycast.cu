@@ -1082,6 +1082,105 @@ hp2_contact_kernel(const __grid_constant__ AgxHp2Scene sc, const __grid_constant
     agx::contact_env(P, rs, cp, n, f, crashes + e);
 }
 
+// hp2_contact_kernel's contact search for one env (centre c), as a function: the nearest contacts in cp / key / id, their count
+// returned.  hp2_contact_kernel keeps its inline copy so that its machine code stays as it was verified: inlining this function
+// there lays out its stack frame differently.
+__device__ __forceinline__ int contact_search(const AgxHp2Scene& sc, const AgxContactParams& P, int e, v3 c, agx::ContactPt* cp, float* key,
+                                              int* id) {
+    const float reach = P.radius + P.contact_offset;
+    const float search = reach * reach;
+    int n = 0;
+    const int K = sc.num_objects;
+    if (K > 0) {
+        const int P2 = sc.leaves_pow2, L = sc.tris_per_object;
+        const float* nodes = sc.nodes + (size_t)e * (2 * P2 - 1) * kNodeFloats;
+        const int32_t* leaf = sc.leaf_object + (size_t)e * (P2 < 4 ? 4 : P2);
+        const float* tris = sc.tris + (size_t)e * K * L * kTriFloats;
+        int stack[24];
+        int sp = 0, node = 0;
+        while (true) {
+            const float* nd = nodes + (size_t)node * kNodeFloats;
+            float dx = fmaxf(fmaxf(nd[0] - c.x, c.x - nd[4]), 0.0f);
+            float dy = fmaxf(fmaxf(nd[1] - c.y, c.y - nd[5]), 0.0f);
+            float dz = fmaxf(fmaxf(nd[2] - c.z, c.z - nd[6]), 0.0f);
+            float box_d2 = dx * dx + dy * dy + dz * dz;
+            if (box_d2 <= search * 1.0001f + 1e-6f) {  // padded boxes + slack: culling only
+                if (node >= P2 - 1) {
+                    const int obj = leaf[node - (P2 - 1)];
+                    ObjClosest best{3.0e38f, v3{0.0f, 0.0f, 0.0f}, nullptr};
+                    if (obj >= 0 && sc.num_meshes && sc.obj_mesh_slot[((size_t)e * K + obj) * 2] >= 0) {
+                        mesh_closest(sc, mesh_ctx(sc, e), obj, c, search, best);
+                    } else if (obj >= 0) {
+                        const float4* tp = reinterpret_cast<const float4*>(tris + (size_t)obj * L * kTriFloats);
+                        for (int s = 0; s < L; ++s) {
+                            const float4 b = tp[3 * s + 1], cc = tp[3 * s + 2];
+                            if (b.x == 0.f && b.y == 0.f && b.z == 0.f && cc.x == 0.f && cc.y == 0.f && cc.z == 0.f) continue;  // padding
+                            tri_closest(c, tp + 3 * s, best);
+                        }
+                    }
+                    if (best.d2 <= search) {
+                        const float dist = sqrtf(best.d2);
+                        v3 nv;
+                        if (dist > 0.0f) {
+                            const v3 d = sub3(c, best.q);
+                            nv = v3{d.x / dist, d.y / dist, d.z / dist};
+                        } else {  // the centre lies on the surface: the triangle's face normal
+                            const float4 b = best.tri[1], cc = best.tri[2];
+                            nv = normalize3(cross3(v3{b.x, b.y, b.z}, v3{cc.x, cc.y, cc.z}));
+                        }
+                        const agx::ContactPt pt{{best.q.x, best.q.y, best.q.z}, {nv.x, nv.y, nv.z}, P.radius - dist};
+                        n = agx::contact_insert(cp, key, id, n, pt, dist, obj);
+                    }
+                } else {
+                    stack[sp++] = 2 * node + 2;
+                    node = 2 * node + 1;
+                    continue;
+                }
+            }
+            if (sp == 0) break;
+            node = stack[--sp];
+        }
+    }
+    if (P.ground_plane && c.z <= reach) {
+        const agx::ContactPt pt{{c.x, c.y, 0.0f}, {0.0f, 0.0f, 1.0f}, P.radius - c.z};
+        n = agx::contact_insert(cp, key, id, n, pt, c.z, K);
+    }
+    return n;
+}
+
+// hp2_contact_kernel with moving obstacles: each kept object contact also gets its obstacle's velocity at the contact point, from
+// the row of the asset that owns the object (mo.obj_asset, in range by the caller's contract); the ground's is 0
+__global__ void __launch_bounds__(128)
+hp2_contact_moving_kernel(const __grid_constant__ AgxHp2Scene sc, const __grid_constant__ AgxContactParams P,
+                          const __grid_constant__ AgxContactMotion mo, int num_envs, float* __restrict__ root_state, int stride,
+                          float* __restrict__ force, uint8_t* __restrict__ crashes, int32_t* __restrict__ contact_obj) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= num_envs) return;
+    float* rs = root_state + (size_t)e * stride;
+    agx::ContactPt cp[AGX_CONTACT_MAX];
+    float key[AGX_CONTACT_MAX];
+    int id[AGX_CONTACT_MAX];
+    const int n = contact_search(sc, P, e, v3{rs[0], rs[1], rs[2]}, cp, key, id);
+    if (contact_obj)
+        for (int i = 0; i < AGX_CONTACT_MAX; ++i) contact_obj[(size_t)e * AGX_CONTACT_MAX + i] = i < n ? id[i] : -1;
+    float* f = force + (size_t)e * 3;
+    if (n == 0) {
+        f[0] = f[1] = f[2] = 0.0f;
+        return;
+    }
+    const int K = sc.num_objects;
+    float u[AGX_CONTACT_MAX][3];
+    for (int i = 0; i < n; ++i) {
+        if (id[i] < K) {
+            const int a = mo.obj_asset[(size_t)e * K + id[i]];
+            agx::obstacle_point_vel(mo.asset_state + ((size_t)e * mo.num_assets + a) * mo.asset_stride, cp[i].p, u[i]);
+        } else {
+            u[i][0] = u[i][1] = u[i][2] = 0.0f;
+        }
+    }
+    agx::contact_env<true>(P, rs, cp, n, f, crashes + e, u);
+}
+
 __device__ __forceinline__ float range_epilogue(const AgxHp2Sensor& s, float px) {
     // warp_sensor.py:216-225: two sequential masked assignments, then the division
     if (px > s.max_range) px = s.far_out_of_range_value;
@@ -1377,6 +1476,27 @@ int validate_scene(const AgxHp2Scene* sc) {
     return AGX_OK;
 }
 
+// the argument checks of both contact entry points; *launch = false: valid, nothing to do (no envs)
+int contact_check(const AgxHp2Scene* sc, int num_envs, const AgxContactParams* p, const float* root_state, int root_state_stride,
+                  const float* contact_force, const uint8_t* crashes, bool* launch) {
+    *launch = false;
+    if (sc) {
+        int rc = validate_scene(sc);
+        if (rc) return rc;
+        if (sc->num_envs != num_envs) return agx_set_error(AGX_E_INVALID, "num_envs %d != scene num_envs %d", num_envs, sc->num_envs);
+    }
+    if (!p) return agx_set_error(AGX_E_NULL, "params is NULL");
+    if (num_envs < 0) return agx_set_error(AGX_E_INVALID, "num_envs < 0");
+    if (!(p->radius >= 0.0f) || !(p->contact_offset >= 0.0f) || !(p->dt > 0.0f) || !(p->mass > 0.0f) || !(p->friction >= 0.0f) ||
+        !(p->max_depenetration_velocity >= 0.0f) || p->iterations < 0)
+        return agx_set_error(AGX_E_INVALID, "contact params out of range");
+    if (num_envs == 0) return AGX_OK;
+    if (!root_state || !contact_force || !crashes) return agx_set_error(AGX_E_NULL, "root_state/contact_force/crashes is NULL");
+    if (root_state_stride < 13) return agx_set_error(AGX_E_INVALID, "root_state_stride < 13");
+    *launch = true;
+    return AGX_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1426,22 +1546,28 @@ int agx_hp2_collide(const AgxHp2Scene* sc, const float* robot_pose, int robot_po
 int agx_hp2_contact(const AgxHp2Scene* sc, int num_envs, const AgxContactParams* p, float* root_state, int root_state_stride,
                     float* contact_force, uint8_t* crashes, int32_t* contact_obj, void* stream) {
     AgxHp2Scene none = {};
-    if (sc) {
-        int rc = validate_scene(sc);
-        if (rc) return rc;
-        if (sc->num_envs != num_envs) return agx_set_error(AGX_E_INVALID, "num_envs %d != scene num_envs %d", num_envs, sc->num_envs);
-    }
-    if (!p) return agx_set_error(AGX_E_NULL, "params is NULL");
-    if (num_envs < 0) return agx_set_error(AGX_E_INVALID, "num_envs < 0");
-    if (!(p->radius >= 0.0f) || !(p->contact_offset >= 0.0f) || !(p->dt > 0.0f) || !(p->mass > 0.0f) || !(p->friction >= 0.0f) ||
-        !(p->max_depenetration_velocity >= 0.0f) || p->iterations < 0)
-        return agx_set_error(AGX_E_INVALID, "contact params out of range");
-    if (num_envs == 0) return AGX_OK;
-    if (!root_state || !contact_force || !crashes) return agx_set_error(AGX_E_NULL, "root_state/contact_force/crashes is NULL");
-    if (root_state_stride < 13) return agx_set_error(AGX_E_INVALID, "root_state_stride < 13");
+    bool launch;
+    int rc = contact_check(sc, num_envs, p, root_state, root_state_stride, contact_force, crashes, &launch);
+    if (rc || !launch) return rc;
     hp2_contact_kernel<<<(num_envs + 127) / 128, 128, 0, (cudaStream_t)stream>>>(sc ? *sc : none, *p, num_envs, root_state,
                                                                                   root_state_stride, contact_force, crashes, contact_obj);
     return agx_check_launch("hp2_contact_kernel");
+}
+
+int agx_hp2_contact_moving(const AgxHp2Scene* sc, int num_envs, const AgxContactParams* p, const AgxContactMotion* m, float* root_state,
+                           int root_state_stride, float* contact_force, uint8_t* crashes, int32_t* contact_obj, void* stream) {
+    if (!sc) return agx_set_error(AGX_E_NULL, "scene is NULL: moving obstacles need a scene");
+    if (!m) return agx_set_error(AGX_E_NULL, "motion is NULL");
+    if (!m->asset_state || !m->obj_asset) return agx_set_error(AGX_E_NULL, "motion asset_state/obj_asset is NULL");
+    if (m->asset_stride < 13) return agx_set_error(AGX_E_INVALID, "motion asset_stride < 13");
+    if (m->num_assets < 1) return agx_set_error(AGX_E_INVALID, "motion num_assets < 1");
+    bool launch;
+    int rc = contact_check(sc, num_envs, p, root_state, root_state_stride, contact_force, crashes, &launch);
+    if (rc || !launch) return rc;
+    hp2_contact_moving_kernel<<<(num_envs + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*sc, *p, *m, num_envs, root_state,
+                                                                                         root_state_stride, contact_force, crashes,
+                                                                                         contact_obj);
+    return agx_check_launch("hp2_contact_moving_kernel");
 }
 
 int agx_hp2_cast(const AgxHp2Scene* sc, const AgxHp2Sensor* sn, void* stream) {

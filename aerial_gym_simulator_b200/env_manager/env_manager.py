@@ -15,6 +15,13 @@ Differences that are deliberate and documented (DESIGN.md):
         sphere at the obstacles and, with ``create_ground_plane``, at the plane z = 0.  It fills ``robot_contact_force_tensor``,
         flags crashes by the reference's rule |F| > collision_force_threshold and adds the force to the IMU's force input.
         args['contact_friction'] is the Coulomb coefficient (default 1.0).  DESIGN.md "Contact mode" has the model.
+        Obstacles are kinematic and, in the solve, at rest: dynamic_env's moving obstacles move once after the n sub-steps.
+      - "rigid" with args['contact_moving_obstacles'] = True: in an env step with env_actions, every sub-step first advances the
+        obstacles by one sub-step and re-poses the scene, then runs the robot's physics sub-step and the contact solve
+        (agx_hp2_contact_moving), which works on the robot's velocity relative to each obstacle's velocity at the contact point.
+        A moving obstacle pushes the robot, carries it by friction and flags a crash by the same force rule.  Obstacles are not
+        pushed back.  The scene is re-posed every sub-step whatever args['refit_dynamic_obstacles'] says.  Steps without
+        env_actions run as in plain "rigid" mode.
 """
 from __future__ import annotations
 
@@ -31,7 +38,7 @@ from .. import _lib
 from .. import robots  # noqa: F401  (registers robots + controllers)
 from .. import urdf
 from ..hp1 import Hp1Engine
-from ..hp2 import RayScene, RaySensor
+from ..hp2 import ContactMotion, RayScene, RaySensor
 from ..hp2 import contact as hp2_contact
 from ..registry._core import env_config_registry, robot_registry, sim_config_registry
 
@@ -111,6 +118,12 @@ class EnvManager:
         if isinstance(mu, bool) or not isinstance(mu, (int, float)) or not math.isfinite(mu) or mu < 0:
             raise ValueError("args['contact_friction'] must be a finite number >= 0")
         self.contact_friction = float(mu)
+        moving = self.env_args.get("contact_moving_obstacles", False)
+        if not isinstance(moving, bool):
+            raise ValueError("args['contact_moving_obstacles'] must be a bool")
+        if moving and self.contact_mode != "rigid":
+            raise ValueError("args['contact_moving_obstacles'] needs args['contact'] = 'rigid'")
+        self.contact_moving_obstacles = moving
         self.global_tensor_dict = {}
         self.step_counter = 0
         self._graphs, self._dist_ctr_dev = {}, None
@@ -189,6 +202,10 @@ class EnvManager:
             p.friction, p.max_depenetration_velocity = self.contact_friction, float(px.max_depenetration_velocity)
             p.force_threshold = float(self.cfg.env.collision_force_threshold)
             p.iterations, p.ground_plane = int(px.num_position_iterations), int(bool(getattr(self.cfg.env, "create_ground_plane", False)))
+        # the moving-obstacle solve reads the asset rows through the object -> asset map (int32, range-checked once here)
+        self._contact_motion = None
+        if self.contact_moving_obstacles and self.scene is not None:
+            self._contact_motion = ContactMotion(self.global_tensor_dict["env_asset_state_tensor"], self._obj_asset)
 
     # ---- obstacles: AssetLoader.select_assets_for_sim + WarpEnv (asset_loader.py:148-194, warp_env_manager.py)
     def _select_assets(self):
@@ -493,14 +510,15 @@ class EnvManager:
         t = _lerp(-mx[:, 3:6], mx[:, 3:6], torch.rand(N, 3, device=dev)) * occ.unsqueeze(1)
         return torch.cat([f, t], dim=1).contiguous()
 
-    def _graph_for(self, n):
-        """CUDA graph of the n physics sub-steps of one env step (captured once per n): per sub-step ONE physics launch that draws its
-        disturbance in the kernel (AgxHp1Buffers.dist_counter: the draw counter lives in device memory, so a replay draws afresh) and
-        ONE collision launch, then one single-thread kernel that advances the draw counter.  Same kernels, same arithmetic, same
-        draws as the launch-by-launch loop (tests: bit-identical trajectories); every C-ABI call is capture-safe (no allocation, no
-        synchronisation).  Navigation-type envs run 10 sub-steps per env step (config/env_config/env_with_obstacles.py:29-30):
-        ~30 launches become one."""
-        g = self._graphs.get(n)
+    def _graph_for(self, n, moving=False):
+        """CUDA graph of the n physics sub-steps of one env step (captured once per (n, moving)): per sub-step ONE physics launch that
+        draws its disturbance in the kernel (AgxHp1Buffers.dist_counter: the draw counter lives in device memory, so a replay draws
+        afresh) and ONE collision launch, then one single-thread kernel that advances the draw counter.  moving (contact with moving
+        obstacles, an env step with env_actions): each sub-step begins with the obstacle advance and the scene re-pose, which read
+        the persistent gtd["env_actions"].  Same kernels, same arithmetic, same draws as the launch-by-launch loop (tests:
+        bit-identical trajectories); every C-ABI call is capture-safe (no allocation, no synchronisation).  Navigation-type envs run
+        10 sub-steps per env step (config/env_config/env_with_obstacles.py:29-30): ~30 launches become one."""
+        g = self._graphs.get((n, moving))
         if g is not None:
             return g
         eng, a = self.engine, self.global_tensor_dict["robot_actions"]
@@ -513,8 +531,10 @@ class EnvManager:
 
         def body():
             for i in range(n):
+                if moving:
+                    self._move_obstacles_one_substep()
                 eng.physics_step(a, physics_steps=1, dist_counter=self._dist_ctr_dev if dist else None, dist_offset=i)
-                self.compute_observations()
+                self.compute_observations(moving_obstacles=moving)
             if dist and n:
                 _lib.check(lib.agx_counter_add(C.c_void_p(self._dist_ctr_dev.data_ptr()), n,
                                                C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)), "agx_counter_add")
@@ -527,17 +547,23 @@ class EnvManager:
                     None if not dist else self._dist_ctr_dev.clone())
             force = self.global_tensor_dict["robot_contact_force_tensor"]
             keep_force = force.clone()
+            if moving:
+                ast = self.global_tensor_dict["env_asset_state_tensor"]
+                keep_obstacles = (ast.clone(), self._obj_pose.clone())
             body()
             eng.root_state.copy_(keep[0]); eng.motor_thrust.copy_(keep[1]); self.collision_tensor.copy_(keep[2])
             force.copy_(keep_force)
             if dist:
                 self._dist_ctr_dev.copy_(keep[3])
+            if moving:
+                ast.copy_(keep_obstacles[0]); self._obj_pose.copy_(keep_obstacles[1])
+                self.scene.update()
         cur.wait_stream(side)
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g, stream=side):
             body()
         # capturing does not execute: the state is untouched, the caller replays
-        self._graphs[n] = g
+        self._graphs[(n, moving)] = g
         return g
 
     def sample_physics_steps(self):
@@ -553,27 +579,34 @@ class EnvManager:
                 if tuple(env_actions.shape) != want or env_actions.dtype != torch.float32 or env_actions.device.type != self.device.type:
                     raise ValueError(f"env_actions must be a float32 {list(want)} tensor on {self.device} (linear + angular velocity per obstacle)")
             if gtd["env_actions"] is None:
-                gtd["env_actions"], gtd["prev_env_actions"] = env_actions, env_actions.clone()
+                # moving-obstacle contact replays graphs that read this buffer: it must be the manager's own, contiguous
+                first = env_actions.contiguous().clone() if self._contact_motion is not None else env_actions
+                gtd["env_actions"], gtd["prev_env_actions"] = first, env_actions.clone()
             gtd["prev_env_actions"][:] = gtd["env_actions"]
             gtd["env_actions"][:] = env_actions
         n = self.sample_physics_steps()
         gtd["robot_prev_actions"][:] = gtd["robot_actions"]  # robot_manager.py:486-488
         gtd["robot_actions"][:] = actions
         a = gtd["robot_actions"]
+        obstacles_move = env_actions is not None and self.num_obs_in_env > 1
+        # contact with moving obstacles: the obstacles advance inside each sub-step, before the robot's (the reference's order)
+        moving = obstacles_move and self._contact_motion is not None
         if self.spec.enable_disturbance or self.scene is not None or self.contact_params is not None:
             # the reference loop (env_manager.py:426-428): fresh disturbance draws and a collision check (or contact solve) after
             # EVERY physics step
             if self.step_mode == "graph":
-                self._graph_for(n).replay()  # the n x (physics launch with in-kernel draw, collision launch) of this env step: one graph launch
+                self._graph_for(n, moving).replay()  # the n x (physics launch with in-kernel draw, collision launch) of this env step: one graph launch
                 if self.spec.enable_disturbance:
                     self._dist_counter += n
             else:
                 for i in range(n):
+                    if moving:
+                        self._move_obstacles_one_substep()
                     self.engine.physics_step(a, disturbance=self._draw_disturbance(), physics_steps=1)
-                    self.compute_observations()
+                    self.compute_observations(moving_obstacles=moving)
         elif n > 0:
             self.engine.physics_step(a, physics_steps=n)  # n sub-steps fused in one launch
-        if env_actions is not None and self.num_obs_in_env > 1 and n > 0:  # ObstacleManager.pre_physics_step, obstacle_manager.py:40-44
+        if obstacles_move and not moving and n > 0:  # ObstacleManager.pre_physics_step, obstacle_manager.py:40-44
             self._step_obstacles(gtd["env_actions"], n)
         self.engine.sim_steps += 1
         self.step_counter += 1
@@ -603,6 +636,11 @@ class EnvManager:
         The reference leaves its Warp meshes stale until the next reset ("refit() ... expensive", env_manager.py:340-342);
         here re-posing + rebuilding the BVHs of all envs is one more launch, done by default (args['refit_dynamic_obstacles'])
         so the ray-cast sensors and the collision test of the next env step see the obstacles where they are."""
+        self._advance_obstacles(twist, n)
+        if self.scene is not None and bool(self.env_args.get("refit_dynamic_obstacles", True)):
+            self._repose_scene()
+
+    def _advance_obstacles(self, twist, n):
         gtd, N, A = self.global_tensor_dict, self.num_envs, self.num_obs_in_env
         ast = gtd["env_asset_state_tensor"]
         twist = twist.contiguous()  # shape / dtype / device were checked in step()
@@ -610,18 +648,26 @@ class EnvManager:
         _lib.check(_lib.load().agx_obstacle_step(N, A, C.c_void_p(ast.data_ptr()), ast.stride(1), C.c_void_p(twist.data_ptr()),
                                                  float(self.sim_config.sim.dt), int(n), self._asset_damping[0], self._asset_damping[1],
                                                  stream), "agx_obstacle_step")
-        if self.scene is not None and bool(self.env_args.get("refit_dynamic_obstacles", True)):
-            idx = self._obj_asset.unsqueeze(-1).expand(-1, -1, 7)
-            self._obj_pose.copy_(torch.gather(ast[..., 0:7], 1, idx))
-            self.scene.update()
 
-    def compute_observations(self):
+    def _repose_scene(self):
+        idx = self._obj_asset.unsqueeze(-1).expand(-1, -1, 7)
+        self._obj_pose.copy_(torch.gather(self.global_tensor_dict["env_asset_state_tensor"][..., 0:7], 1, idx))
+        self.scene.update()
+
+    def _move_obstacles_one_substep(self):
+        """contact with moving obstacles: one sub-step of the obstacles (the advance keeps its state in float32, so n of these add
+        up bit for bit to one n-sub-step advance) and the scene re-posed where they now are"""
+        self._advance_obstacles(self.global_tensor_dict["env_actions"], 1)
+        self._repose_scene()
+
+    def compute_observations(self, moving_obstacles=False):
         """crashes += contact (env_manager.py:358-362).  PhysX contact forces are replaced by a
         geometric test: the base-link collision sphere overlaps the env mesh (agx_hp2_collide).  Contact mode: the contact solve
-        (agx_hp2_contact) in its place, which flags by the contact force as the reference does."""
+        (agx_hp2_contact) in its place, which flags by the contact force as the reference does.  moving_obstacles: the solve takes
+        the obstacles' velocities (agx_hp2_contact_moving; only with args['contact_moving_obstacles'])."""
         if self.contact_params is not None:
             hp2_contact(self.scene, self.engine.root_state, self.contact_params, self.global_tensor_dict["robot_contact_force_tensor"],
-                        self.collision_tensor)
+                        self.collision_tensor, motion=self._contact_motion if moving_obstacles else None)
         elif self.scene is not None:
             self.scene.collide(self.engine.root_state, self.robot.collision_radius, self.collision_tensor)
 

@@ -266,16 +266,43 @@ class RayScene:
                    "agx_hp2_collide")
 
     def contact(self, robot_state: torch.Tensor, params: _lib.AgxContactParams, force: torch.Tensor, crashes: torch.Tensor,
-                contact_obj: Optional[torch.Tensor] = None):
+                contact_obj: Optional[torch.Tensor] = None, motion: Optional["ContactMotion"] = None):
         """One rigid-contact solve against this scene (and the ground plane if params.ground_plane): see contact()."""
-        contact(self, robot_state, params, force, crashes, contact_obj)
+        contact(self, robot_state, params, force, crashes, contact_obj, motion)
+
+
+class ContactMotion:
+    """What the moving-obstacle contact solve (agx_hp2_contact_moving) reads of the obstacles.
+    asset_state: float32 [E,A,>=13] device tensor (env_asset_state_tensor: x y z, q xyzw, world linear and angular velocity per
+    asset), rows uniformly strided with a contiguous last dim; read at every solve, so it may change between solves.
+    obj_asset: integer [E,K]: the asset each scene object belongs to, every value in [0, A).  Checked here once (one host read), so
+    that the solves themselves never synchronise with the host; kept as a contiguous int32 device copy."""
+
+    def __init__(self, asset_state: torch.Tensor, obj_asset: torch.Tensor):
+        if not isinstance(asset_state, torch.Tensor) or asset_state.dtype != torch.float32 or asset_state.dim() != 3 \
+                or asset_state.shape[2] < 13 or asset_state.shape[1] < 1:
+            raise ValueError("asset_state must be a float32 [E,A>=1,>=13] tensor")
+        if asset_state.stride(2) != 1 or asset_state.stride(0) != asset_state.shape[1] * asset_state.stride(1):
+            raise ValueError("asset_state rows must be uniformly strided with a contiguous last dim")
+        if not isinstance(obj_asset, torch.Tensor) or obj_asset.dtype not in (torch.int32, torch.int64) or obj_asset.dim() != 2 \
+                or obj_asset.shape[0] != asset_state.shape[0] or obj_asset.device != asset_state.device:
+            raise ValueError("obj_asset must be an integer [E,K] tensor on asset_state's device, E = asset_state.shape[0]")
+        A = asset_state.shape[1]
+        if obj_asset.numel() and (int(obj_asset.min()) < 0 or int(obj_asset.max()) >= A):
+            raise ValueError(f"obj_asset values must be in [0, {A})")
+        self.asset_state, self.obj_asset = asset_state, obj_asset.to(torch.int32).contiguous()
+        self.E, self.K, self.device = obj_asset.shape[0], obj_asset.shape[1], asset_state.device
+        self.c = _lib.AgxContactMotion(asset_state=asset_state.data_ptr(), asset_stride=asset_state.stride(1), num_assets=A,
+                                       obj_asset=self.obj_asset.data_ptr())
 
 
 def contact(scene: Optional[RayScene], robot_state: torch.Tensor, params: _lib.AgxContactParams, force: torch.Tensor,
-            crashes: torch.Tensor, contact_obj: Optional[torch.Tensor] = None):
+            crashes: torch.Tensor, contact_obj: Optional[torch.Tensor] = None, motion: Optional[ContactMotion] = None):
     """agx_hp2_contact: the robot's collision sphere against the scene's objects (scene None: none) and the ground plane.
     robot_state [E,>=13] float32: linear and world angular velocity updated in place; force [E,3] float32 = contact impulse / dt;
-    crashes (bool [E]) |= |force| > params.force_threshold; contact_obj (int32 [E,CONTACT_MAX], optional) = contacts used."""
+    crashes (bool [E]) |= |force| > params.force_threshold; contact_obj (int32 [E,CONTACT_MAX], optional) = contacts used.
+    motion (ContactMotion of this scene's objects, optional): the obstacles move; the solve works on the robot's velocity relative to
+    each obstacle's velocity at the contact point (agx_hp2_contact_moving).  None: every obstacle is at rest (agx_hp2_contact)."""
     E = robot_state.shape[0]
     dev = robot_state.device
     if dev.type != "cuda":
@@ -291,8 +318,21 @@ def contact(scene: Optional[RayScene], robot_state: torch.Tensor, params: _lib.A
     if contact_obj is not None and (contact_obj.dtype != torch.int32 or contact_obj.shape != (E, _lib.CONTACT_MAX)
                                     or not contact_obj.is_contiguous() or contact_obj.device != dev):
         raise ValueError(f"contact_obj must be contiguous int32 [E,{_lib.CONTACT_MAX}]")
+    if motion is not None:
+        if not isinstance(motion, ContactMotion):
+            raise ValueError("motion must be a ContactMotion")
+        if scene is None:
+            raise ValueError("moving obstacles need a scene")
+        if (motion.E, motion.K) != (scene.E, scene.K) or motion.device != dev:
+            raise ValueError("motion must map this scene's [E,K] objects, on the scene's device")
     lib = _lib.load()
     co = C.c_void_p(contact_obj.data_ptr()) if contact_obj is not None else None
+    stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    if motion is not None:
+        _lib.check(lib.agx_hp2_contact_moving(C.byref(scene.c), E, C.byref(params), C.byref(motion.c), C.c_void_p(robot_state.data_ptr()),
+                                              robot_state.stride(0), C.c_void_p(force.data_ptr()), C.c_void_p(crashes.data_ptr()), co,
+                                              stream), "agx_hp2_contact_moving")
+        return
     _lib.check(lib.agx_hp2_contact(C.byref(scene.c) if scene is not None else None, E, C.byref(params),
                                    C.c_void_p(robot_state.data_ptr()), robot_state.stride(0), C.c_void_p(force.data_ptr()),
                                    C.c_void_p(crashes.data_ptr()), co, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),

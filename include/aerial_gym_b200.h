@@ -173,7 +173,7 @@ const char* agx_last_error(void);
 /* sizeof() of the ABI structs as compiled into the library (binding self-check):
  * which = 0 AgxHp1Config, 1 AgxHp1Buffers, 2 AgxHp1ResetDraws, 3 AgxHp2Scene, 4 AgxHp2Sensor,
  * 5 AgxNavRewardParams, 6 AgxImuConfig, 7 AgxLidarNavRewardParams, 8 AgxHp2Noise, 9 AgxE2ERewardParams, 10 AgxObsGatherPush,
- * 11 AgxContactParams */
+ * 11 AgxContactParams, 12 AgxContactMotion */
 uint64_t agx_sizeof(int which);
 
 /* Host buffers the kernels can address directly (pinned, portable, mapped: cudaHostAlloc).
@@ -527,7 +527,8 @@ int agx_hp2_collide(const AgxHp2Scene* scene, const float* robot_pose, int robot
  * with ground_plane, the plane z = 0 (normal +z); the AGX_CONTACT_MAX nearest are kept, ties to the lower object index, the
  * ground last.  One sequential-impulse solve (`iterations` passes; per contact a normal impulse >= 0 with target separating
  * velocity min(max(depth - rest_offset, 0) / dt, max_depenetration_velocity), then Coulomb friction with a circular clamp
- * |lambda_t| <= friction * lambda_n).  Obstacles are kinematic and at rest.  Lever arms are taken about p + R com. */
+ * |lambda_t| <= friction * lambda_n).  Obstacles are kinematic (infinite mass); agx_hp2_contact treats them as at rest,
+ * agx_hp2_contact_moving below gives them their velocity.  Lever arms are taken about p + R com. */
 #define AGX_CONTACT_MAX 8
 typedef struct AgxContactParams {
     float radius;               /* robot collision sphere */
@@ -552,6 +553,25 @@ typedef struct AgxContactParams {
  *                             -1 = unused slot) */
 int agx_hp2_contact(const AgxHp2Scene* scene, int num_envs, const AgxContactParams* params, float* root_state, int root_state_stride,
                     float* contact_force, uint8_t* crashes, int32_t* contact_obj, void* stream);
+
+/* Moving obstacles (DESIGN.md "Contact mode", "Moving obstacles"): the solve above on the robot's velocity relative to the obstacle.
+ * Object k of env e belongs to asset a = obj_asset[e,k]; at contact point p its velocity is u = v_a + w_a x (p - x_a), from the
+ * asset's row (position, world linear and angular velocity).  The normal row targets n . (v_robot(p) - u) >= bias, the friction row
+ * drives the tangential part of v_robot(p) - u to 0; the ground plane has u = 0.  With every u = 0 the arithmetic is
+ * agx_hp2_contact's.  Obstacles are not pushed. */
+typedef struct AgxContactMotion {
+    const float* asset_state;   /* [E,num_assets,asset_stride] rows x y z qx qy qz qw vx vy vz wx wy wz (env_asset_state_tensor) */
+    int32_t asset_stride;       /* >= 13 */
+    int32_t num_assets;
+    const int32_t* obj_asset;   /* [E,num_objects] asset of each scene object; every value in [0, num_assets): the caller checks
+                                   this when it builds the map, the kernel reads without a bounds check */
+} AgxContactMotion;
+
+/* As agx_hp2_contact, with the same arguments and checks, plus `motion` (non-NULL pointers, asset_stride >= 13, num_assets >= 1).
+ * scene must not be NULL. */
+int agx_hp2_contact_moving(const AgxHp2Scene* scene, int num_envs, const AgxContactParams* params, const AgxContactMotion* motion,
+                           float* root_state, int root_state_stride, float* contact_force, uint8_t* crashes, int32_t* contact_obj,
+                           void* stream);
 
 
 /* ======================================================================================
