@@ -147,6 +147,10 @@ class AgxContactMotion(C.Structure):
     _fields_ = [("asset_state", C.c_void_p), ("asset_stride", C.c_int32), ("num_assets", C.c_int32), ("obj_asset", C.c_void_p)]
 
 
+class AgxObstacleMass(C.Structure):
+    _fields_ = [("inv_mass", f32), ("com", f32 * 3), ("inertia_inv", f32 * 9)]
+
+
 SENSOR_CAMERA, SENSOR_LIDAR, SENSOR_STEREO_CAMERA, SENSOR_NORMAL_FACEID_CAMERA, SENSOR_NORMAL_FACEID_LIDAR = 0, 1, 2, 3, 4
 
 
@@ -222,6 +226,8 @@ def load():
                             C.c_void_p, C.c_void_p],
         "agx_hp2_contact_moving": [C.POINTER(AgxHp2Scene), C.c_int, C.POINTER(AgxContactParams), C.POINTER(AgxContactMotion), C.c_void_p,
                                    C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
+        "agx_hp2_contact_dynamic": [C.POINTER(AgxHp2Scene), C.c_int, C.POINTER(AgxContactParams), C.POINTER(AgxContactMotion), C.c_void_p,
+                                    C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
     }.items():
         try:
             fn = getattr(lib, name)
@@ -237,7 +243,7 @@ def load():
     if lib.agx_sizeof(5) != C.sizeof(AgxNavRewardParams) or lib.agx_sizeof(6) != C.sizeof(AgxImuConfig) \
             or lib.agx_sizeof(7) != C.sizeof(AgxLidarNavRewardParams) or lib.agx_sizeof(8) != C.sizeof(AgxHp2Noise) \
             or lib.agx_sizeof(9) != C.sizeof(AgxE2ERewardParams) or lib.agx_sizeof(11) != C.sizeof(AgxContactParams) \
-            or lib.agx_sizeof(12) != C.sizeof(AgxContactMotion):
+            or lib.agx_sizeof(12) != C.sizeof(AgxContactMotion) or lib.agx_sizeof(13) != C.sizeof(AgxObstacleMass):
         raise AgxError("aux ABI struct size mismatch between _lib.py and libaerial_gym_b200.so")
     if lib.agx_sizeof(0) != C.sizeof(AgxHp1Config) or lib.agx_sizeof(1) != C.sizeof(AgxHp1Buffers) \
             or lib.agx_sizeof(2) != C.sizeof(AgxHp1ResetDraws) or lib.agx_sizeof(10) != C.sizeof(AgxObsGatherPush):

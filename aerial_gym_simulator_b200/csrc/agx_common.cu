@@ -62,6 +62,7 @@ uint64_t agx_sizeof(int which) {
         case 8: return sizeof(AgxHp2Noise);
         case 11: return sizeof(AgxContactParams);
         case 12: return sizeof(AgxContactMotion);
+        case 13: return sizeof(AgxObstacleMass);
 #endif
         default: return 0;
     }

@@ -1181,6 +1181,37 @@ hp2_contact_moving_kernel(const __grid_constant__ AgxHp2Scene sc, const __grid_c
     agx::contact_env<true>(P, rs, cp, n, f, crashes + e, u);
 }
 
+// hp2_contact_moving_kernel with dynamic obstacles: the assets of the kept object contacts become the bodies of the two-body solve
+// (at most AGX_CONTACT_MAX per env, one per distinct asset, in the order of their first contact), loaded from their rows and mass
+// entries, solved with the robot, and the free ones written back to their rows.  Only this env's thread touches this env's rows.
+__global__ void __launch_bounds__(128)
+hp2_contact_dynamic_kernel(const __grid_constant__ AgxHp2Scene sc, const __grid_constant__ AgxContactParams P,
+                           const __grid_constant__ AgxContactMotion mo, float* __restrict__ asset_state,
+                           const AgxObstacleMass* __restrict__ mass, int num_envs, float* __restrict__ root_state, int stride,
+                           float* __restrict__ force, uint8_t* __restrict__ crashes, int32_t* __restrict__ contact_obj) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= num_envs) return;
+    float* rs = root_state + (size_t)e * stride;
+    agx::ContactPt cp[AGX_CONTACT_MAX];
+    float key[AGX_CONTACT_MAX];
+    int id[AGX_CONTACT_MAX];
+    const int n = contact_search(sc, P, e, v3{rs[0], rs[1], rs[2]}, cp, key, id);
+    if (contact_obj)
+        for (int i = 0; i < AGX_CONTACT_MAX; ++i) contact_obj[(size_t)e * AGX_CONTACT_MAX + i] = i < n ? id[i] : -1;
+    float* f = force + (size_t)e * 3;
+    if (n == 0) {
+        f[0] = f[1] = f[2] = 0.0f;
+        return;
+    }
+    const int K = sc.num_objects, A = mo.num_assets;
+    agx::ContactBody B[AGX_CONTACT_MAX];
+    float* rows[AGX_CONTACT_MAX];
+    int body[AGX_CONTACT_MAX];
+    const int nb = agx::contact_bodies_gather(id, n, K, mo.obj_asset + (size_t)e * K, asset_state + (size_t)e * A * mo.asset_stride,
+                                              mo.asset_stride, mass + (size_t)e * A, B, rows, body);
+    agx::contact_env_dynamic(P, rs, cp, n, f, crashes + e, body, B, nb, rows);
+}
+
 __device__ __forceinline__ float range_epilogue(const AgxHp2Sensor& s, float px) {
     // warp_sensor.py:216-225: two sequential masked assignments, then the division
     if (px > s.max_range) px = s.far_out_of_range_value;
@@ -1568,6 +1599,26 @@ int agx_hp2_contact_moving(const AgxHp2Scene* sc, int num_envs, const AgxContact
                                                                                          root_state_stride, contact_force, crashes,
                                                                                          contact_obj);
     return agx_check_launch("hp2_contact_moving_kernel");
+}
+
+int agx_hp2_contact_dynamic(const AgxHp2Scene* sc, int num_envs, const AgxContactParams* p, const AgxContactMotion* m,
+                            const AgxObstacleMass* mass, float* root_state, int root_state_stride, float* contact_force, uint8_t* crashes,
+                            int32_t* contact_obj, void* stream) {
+    if (!sc) return agx_set_error(AGX_E_NULL, "scene is NULL: dynamic obstacles need a scene");
+    if (!m) return agx_set_error(AGX_E_NULL, "motion is NULL");
+    if (!m->asset_state || !m->obj_asset) return agx_set_error(AGX_E_NULL, "motion asset_state/obj_asset is NULL");
+    if (m->asset_stride < 13) return agx_set_error(AGX_E_INVALID, "motion asset_stride < 13");
+    if (m->num_assets < 1) return agx_set_error(AGX_E_INVALID, "motion num_assets < 1");
+    if (!mass) return agx_set_error(AGX_E_NULL, "mass is NULL");
+    bool launch;
+    int rc = contact_check(sc, num_envs, p, root_state, root_state_stride, contact_force, crashes, &launch);
+    if (rc || !launch) return rc;
+    // the rows are written back: the caller's contract (aerial_gym_b200.h) is a writable asset_state buffer
+    float* asset_state = const_cast<float*>(m->asset_state);
+    hp2_contact_dynamic_kernel<<<(num_envs + 127) / 128, 128, 0, (cudaStream_t)stream>>>(*sc, *p, *m, asset_state, mass, num_envs,
+                                                                                          root_state, root_state_stride, contact_force,
+                                                                                          crashes, contact_obj);
+    return agx_check_launch("hp2_contact_dynamic_kernel");
 }
 
 int agx_hp2_cast(const AgxHp2Scene* sc, const AgxHp2Sensor* sn, void* stream) {

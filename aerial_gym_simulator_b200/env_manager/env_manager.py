@@ -22,6 +22,11 @@ Differences that are deliberate and documented (DESIGN.md):
         A moving obstacle pushes the robot, carries it by friction and flags a crash by the same force rule.  Obstacles are not
         pushed back.  The scene is re-posed every sub-step whatever args['refit_dynamic_obstacles'] says.  Steps without
         env_actions run as in plain "rigid" mode.
+      - ... and args['contact_dynamic_obstacles'] = True: every obstacle asset is a free rigid body with its URDF's mass, COM and
+        inertia (every asset needs fix_base_link = False).  The solve (agx_hp2_contact_dynamic) gives each impulse to the robot and,
+        opposite, to the obstacle, and writes the pushed obstacles' twist and a first-order position correction to their rows.
+        Every sub-step advances the obstacles, in steps without env_actions with their own damped velocity, so a knocked obstacle
+        drifts; the scene is re-posed once more after the last sub-step; reset_idx zeroes the reset envs' obstacle velocities.
 """
 from __future__ import annotations
 
@@ -38,7 +43,7 @@ from .. import _lib
 from .. import robots  # noqa: F401  (registers robots + controllers)
 from .. import urdf
 from ..hp1 import Hp1Engine
-from ..hp2 import ContactMotion, RayScene, RaySensor
+from ..hp2 import ContactMotion, ObstacleMass, RayScene, RaySensor
 from ..hp2 import contact as hp2_contact
 from ..registry._core import env_config_registry, robot_registry, sim_config_registry
 
@@ -54,6 +59,17 @@ def _quat_from_euler(e):  # utils/math.py:155-172
     cp, sp = torch.cos(pitch * 0.5), torch.sin(pitch * 0.5)
     return torch.stack([cy * sr * cp - sy * cr * sp, cy * cr * sp + sy * sr * cp, sy * cr * cp - cy * sr * sp,
                         cy * cr * cp + sy * sr * sp], dim=-1)
+
+
+def _obstacle_mass_row(model, path):
+    """the AgxObstacleMass row of a free obstacle asset: the composite mass properties of its URDF inertials (the robot's come from
+    the same function).  No density is assumed: an asset without mass is an error."""
+    m, com, J = model.composite_inertia()
+    if not m > 0:
+        raise ValueError(f"{path}: a free obstacle asset needs URDF inertials with a total mass > 0")
+    if not np.linalg.matrix_rank(J) == 3:
+        raise ValueError(f"{path}: the composite inertia of a free obstacle asset must be invertible")
+    return ObstacleMass.row(m, com, J)
 
 
 def _quat_rotate_inverse(q, v):
@@ -124,6 +140,12 @@ class EnvManager:
         if moving and self.contact_mode != "rigid":
             raise ValueError("args['contact_moving_obstacles'] needs args['contact'] = 'rigid'")
         self.contact_moving_obstacles = moving
+        dynamic = self.env_args.get("contact_dynamic_obstacles", False)
+        if not isinstance(dynamic, bool):
+            raise ValueError("args['contact_dynamic_obstacles'] must be a bool")
+        if dynamic and not moving:
+            raise ValueError("args['contact_dynamic_obstacles'] needs args['contact_moving_obstacles'] = True")
+        self.contact_dynamic_obstacles = dynamic
         self.global_tensor_dict = {}
         self.step_counter = 0
         self._graphs, self._dist_ctr_dev = {}, None
@@ -206,6 +228,10 @@ class EnvManager:
         self._contact_motion = None
         if self.contact_moving_obstacles and self.scene is not None:
             self._contact_motion = ContactMotion(self.global_tensor_dict["env_asset_state_tensor"], self._obj_asset)
+        # the dynamic-obstacle solve: every asset a free body with its URDF's mass properties (table built in _build_obstacles)
+        self._obstacle_mass = None
+        if self._contact_motion is not None and self.contact_dynamic_obstacles:
+            self._obstacle_mass = ObstacleMass(self._asset_mass.to(dev))
 
     # ---- obstacles: AssetLoader.select_assets_for_sim + WarpEnv (asset_loader.py:148-194, warp_env_manager.py)
     def _select_assets(self):
@@ -270,11 +296,19 @@ class EnvManager:
         # every cluster template (RayScene's mesh_templates).
         templates, tmpl_obbs, boxes_of, tmpl_link = [], [], {}, []
         meshes, mesh_link = [], []
+        # dynamic obstacles: one mass-table row per distinct URDF (inverse mass, COM, inverse inertia: AgxObstacleMass)
+        dynamic = self.contact_dynamic_obstacles
+        mass_of, asset_mass = {}, (np.zeros((N, A, 13), np.float32) if dynamic else None)
         for e in range(N):
             for a, (params, path) in enumerate(per_env[e]):
                 lo[e, a], hi[e, a] = params.min_state_ratio, params.max_state_ratio
+                if dynamic and getattr(params, "fix_base_link", True):
+                    raise ValueError(f"args['contact_dynamic_obstacles'] needs every obstacle asset to have fix_base_link = False "
+                                     f"({getattr(params, '__name__', type(params).__name__)} has a fixed base link)")
                 if path not in boxes_of:
                     model = urdf.parse_urdf(path)
+                    if dynamic:
+                        mass_of[path] = _obstacle_mass_row(model, path)
                     ids = []
                     for _, link_index, tris, obb in urdf.visual_parts(model, params.use_collision_mesh_instead_of_visual):
                         if obb is None:
@@ -287,6 +321,10 @@ class EnvManager:
                         tmpl_obbs.append(obb)
                         tmpl_link.append(link_index)
                     boxes_of[path] = ids
+                if dynamic:
+                    asset_mass[e, a] = mass_of[path]
+        if dynamic:
+            self._asset_mass = torch.from_numpy(asset_mass)
         gtd["asset_min_state_ratio"].copy_(torch.from_numpy(lo))
         gtd["asset_max_state_ratio"].copy_(torch.from_numpy(hi))
         if not self.use_warp:
@@ -468,6 +506,9 @@ class EnvManager:
         if len(sel) > 0:
             self._reset_assets(env_ids[sel], A // 2)
         self._num_keep = self.keep_in_env
+        if self._obstacle_mass is not None:
+            # free obstacles keep the twist the contact solve gave them: the reset writes the state ratios' zero velocities
+            gtd["env_asset_state_tensor"][env_ids, :, 7:13] = 0.0
         if self.scene is not None:  # WarpEnv.reset_idx (warp_env_manager.py:40-54)
             idx = self._obj_asset.unsqueeze(-1).expand(-1, -1, 7)
             self._obj_pose.copy_(torch.gather(gtd["env_asset_state_tensor"][..., 0:7], 1, idx))
@@ -517,12 +558,16 @@ class EnvManager:
         obstacles, an env step with env_actions): each sub-step begins with the obstacle advance and the scene re-pose, which read
         the persistent gtd["env_actions"].  Same kernels, same arithmetic, same draws as the launch-by-launch loop (tests:
         bit-identical trajectories); every C-ABI call is capture-safe (no allocation, no synchronisation).  Navigation-type envs run
-        10 sub-steps per env step (config/env_config/env_with_obstacles.py:29-30): ~30 launches become one."""
+        10 sub-steps per env step (config/env_config/env_with_obstacles.py:29-30): ~30 launches become one.
+        Dynamic obstacles (args['contact_dynamic_obstacles'], fixed for the manager, so (n, moving) keys the graph): every sub-step
+        advances the obstacles, with the env_actions twist when moving and with their own velocity otherwise, the solve writes the
+        obstacles it pushes, and the scene is re-posed once more after the last sub-step."""
         g = self._graphs.get((n, moving))
         if g is not None:
             return g
         eng, a = self.engine, self.global_tensor_dict["robot_actions"]
         dist = self.spec.enable_disturbance
+        dynamic = self._obstacle_mass is not None
         if dist and self._dist_ctr_dev is None:
             self._draw_disturbance()  # creates the stream state (seed, counters); the draw itself is discarded ...
             self._dist_counter -= 1   # ... and not counted
@@ -531,10 +576,12 @@ class EnvManager:
 
         def body():
             for i in range(n):
-                if moving:
-                    self._move_obstacles_one_substep()
+                if moving or dynamic:
+                    self._move_obstacles_one_substep(with_twist=moving)
                 eng.physics_step(a, physics_steps=1, dist_counter=self._dist_ctr_dev if dist else None, dist_offset=i)
-                self.compute_observations(moving_obstacles=moving)
+                self.compute_observations(moving_obstacles=moving or dynamic)
+            if dynamic and n:
+                self._repose_scene()
             if dist and n:
                 _lib.check(lib.agx_counter_add(C.c_void_p(self._dist_ctr_dev.data_ptr()), n,
                                                C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)), "agx_counter_add")
@@ -547,7 +594,7 @@ class EnvManager:
                     None if not dist else self._dist_ctr_dev.clone())
             force = self.global_tensor_dict["robot_contact_force_tensor"]
             keep_force = force.clone()
-            if moving:
+            if moving or dynamic:
                 ast = self.global_tensor_dict["env_asset_state_tensor"]
                 keep_obstacles = (ast.clone(), self._obj_pose.clone())
             body()
@@ -555,7 +602,7 @@ class EnvManager:
             force.copy_(keep_force)
             if dist:
                 self._dist_ctr_dev.copy_(keep[3])
-            if moving:
+            if moving or dynamic:
                 ast.copy_(keep_obstacles[0]); self._obj_pose.copy_(keep_obstacles[1])
                 self.scene.update()
         cur.wait_stream(side)
@@ -591,6 +638,8 @@ class EnvManager:
         obstacles_move = env_actions is not None and self.num_obs_in_env > 1
         # contact with moving obstacles: the obstacles advance inside each sub-step, before the robot's (the reference's order)
         moving = obstacles_move and self._contact_motion is not None
+        # dynamic obstacles: free bodies that also drift (and get pushed) in steps without env_actions
+        dynamic = self._obstacle_mass is not None
         if self.spec.enable_disturbance or self.scene is not None or self.contact_params is not None:
             # the reference loop (env_manager.py:426-428): fresh disturbance draws and a collision check (or contact solve) after
             # EVERY physics step
@@ -600,10 +649,12 @@ class EnvManager:
                     self._dist_counter += n
             else:
                 for i in range(n):
-                    if moving:
-                        self._move_obstacles_one_substep()
+                    if moving or dynamic:
+                        self._move_obstacles_one_substep(with_twist=moving)
                     self.engine.physics_step(a, disturbance=self._draw_disturbance(), physics_steps=1)
-                    self.compute_observations(moving_obstacles=moving)
+                    self.compute_observations(moving_obstacles=moving or dynamic)
+                if dynamic and n:  # the solve moved the obstacles it pushed: sensors and the next step see them there
+                    self._repose_scene()
         elif n > 0:
             self.engine.physics_step(a, physics_steps=n)  # n sub-steps fused in one launch
         if obstacles_move and not moving and n > 0:  # ObstacleManager.pre_physics_step, obstacle_manager.py:40-44
@@ -643,9 +694,10 @@ class EnvManager:
     def _advance_obstacles(self, twist, n):
         gtd, N, A = self.global_tensor_dict, self.num_envs, self.num_obs_in_env
         ast = gtd["env_asset_state_tensor"]
-        twist = twist.contiguous()  # shape / dtype / device were checked in step()
+        twist = twist.contiguous() if twist is not None else None  # shape / dtype / device were checked in step(); None: own velocity
         stream = C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-        _lib.check(_lib.load().agx_obstacle_step(N, A, C.c_void_p(ast.data_ptr()), ast.stride(1), C.c_void_p(twist.data_ptr()),
+        tw = C.c_void_p(twist.data_ptr()) if twist is not None else None
+        _lib.check(_lib.load().agx_obstacle_step(N, A, C.c_void_p(ast.data_ptr()), ast.stride(1), tw,
                                                  float(self.sim_config.sim.dt), int(n), self._asset_damping[0], self._asset_damping[1],
                                                  stream), "agx_obstacle_step")
 
@@ -654,20 +706,23 @@ class EnvManager:
         self._obj_pose.copy_(torch.gather(self.global_tensor_dict["env_asset_state_tensor"][..., 0:7], 1, idx))
         self.scene.update()
 
-    def _move_obstacles_one_substep(self):
+    def _move_obstacles_one_substep(self, with_twist=True):
         """contact with moving obstacles: one sub-step of the obstacles (the advance keeps its state in float32, so n of these add
-        up bit for bit to one n-sub-step advance) and the scene re-posed where they now are"""
-        self._advance_obstacles(self.global_tensor_dict["env_actions"], 1)
+        up bit for bit to one n-sub-step advance) and the scene re-posed where they now are.  with_twist False (dynamic obstacles in
+        a step without env_actions): each obstacle keeps its own damped velocity."""
+        self._advance_obstacles(self.global_tensor_dict["env_actions"] if with_twist else None, 1)
         self._repose_scene()
 
     def compute_observations(self, moving_obstacles=False):
         """crashes += contact (env_manager.py:358-362).  PhysX contact forces are replaced by a
         geometric test: the base-link collision sphere overlaps the env mesh (agx_hp2_collide).  Contact mode: the contact solve
         (agx_hp2_contact) in its place, which flags by the contact force as the reference does.  moving_obstacles: the solve takes
-        the obstacles' velocities (agx_hp2_contact_moving; only with args['contact_moving_obstacles'])."""
+        the obstacles' velocities (agx_hp2_contact_moving; only with args['contact_moving_obstacles']), and with
+        args['contact_dynamic_obstacles'] also pushes them (agx_hp2_contact_dynamic)."""
         if self.contact_params is not None:
             hp2_contact(self.scene, self.engine.root_state, self.contact_params, self.global_tensor_dict["robot_contact_force_tensor"],
-                        self.collision_tensor, motion=self._contact_motion if moving_obstacles else None)
+                        self.collision_tensor, motion=self._contact_motion if moving_obstacles else None,
+                        mass=self._obstacle_mass if moving_obstacles else None)
         elif self.scene is not None:
             self.scene.collide(self.engine.root_state, self.robot.collision_radius, self.collision_tensor)
 

@@ -266,9 +266,10 @@ class RayScene:
                    "agx_hp2_collide")
 
     def contact(self, robot_state: torch.Tensor, params: _lib.AgxContactParams, force: torch.Tensor, crashes: torch.Tensor,
-                contact_obj: Optional[torch.Tensor] = None, motion: Optional["ContactMotion"] = None):
+                contact_obj: Optional[torch.Tensor] = None, motion: Optional["ContactMotion"] = None,
+                mass: Optional["ObstacleMass"] = None):
         """One rigid-contact solve against this scene (and the ground plane if params.ground_plane): see contact()."""
-        contact(self, robot_state, params, force, crashes, contact_obj, motion)
+        contact(self, robot_state, params, force, crashes, contact_obj, motion, mass)
 
 
 class ContactMotion:
@@ -296,13 +297,41 @@ class ContactMotion:
                                        obj_asset=self.obj_asset.data_ptr())
 
 
+class ObstacleMass:
+    """The per-(env, asset) mass table of the dynamic-obstacle contact solve (agx_hp2_contact_dynamic), one AgxObstacleMass per row.
+    table: float32 [E,A,13] contiguous device tensor: inverse mass, COM in the asset frame (3), inverse inertia about the COM in
+    asset-frame axes (9, row-major).  Checked here once (one host read): finite values, inverse mass >= 0.  An all-zero row is a
+    kinematic asset (infinite mass: the solve reads its twist and never writes its row)."""
+
+    def __init__(self, table: torch.Tensor):
+        if not isinstance(table, torch.Tensor) or table.dtype != torch.float32 or table.dim() != 3 or table.shape[2] != 13 \
+                or table.shape[1] < 1:
+            raise ValueError("the obstacle mass table must be a float32 [E,A>=1,13] tensor")
+        if not table.is_contiguous():
+            raise ValueError("the obstacle mass table must be contiguous")
+        if not bool(torch.isfinite(table).all()):
+            raise ValueError("the obstacle mass table must be finite")
+        if bool((table[..., 0] < 0).any()):
+            raise ValueError("obstacle inverse masses must be >= 0")
+        self.table, self.E, self.A, self.device = table, table.shape[0], table.shape[1], table.device
+
+    @staticmethod
+    def row(mass: float, com, inertia) -> np.ndarray:
+        """one float32 row from a mass, a COM (asset frame) and an inertia about the COM (asset-frame axes)"""
+        return np.concatenate([[1.0 / mass], np.asarray(com, np.float64).reshape(3),
+                               np.linalg.inv(np.asarray(inertia, np.float64).reshape(3, 3)).reshape(9)]).astype(np.float32)
+
+
 def contact(scene: Optional[RayScene], robot_state: torch.Tensor, params: _lib.AgxContactParams, force: torch.Tensor,
-            crashes: torch.Tensor, contact_obj: Optional[torch.Tensor] = None, motion: Optional[ContactMotion] = None):
+            crashes: torch.Tensor, contact_obj: Optional[torch.Tensor] = None, motion: Optional[ContactMotion] = None,
+            mass: Optional[ObstacleMass] = None):
     """agx_hp2_contact: the robot's collision sphere against the scene's objects (scene None: none) and the ground plane.
     robot_state [E,>=13] float32: linear and world angular velocity updated in place; force [E,3] float32 = contact impulse / dt;
     crashes (bool [E]) |= |force| > params.force_threshold; contact_obj (int32 [E,CONTACT_MAX], optional) = contacts used.
     motion (ContactMotion of this scene's objects, optional): the obstacles move; the solve works on the robot's velocity relative to
-    each obstacle's velocity at the contact point (agx_hp2_contact_moving).  None: every obstacle is at rest (agx_hp2_contact)."""
+    each obstacle's velocity at the contact point (agx_hp2_contact_moving).  None: every obstacle is at rest (agx_hp2_contact).
+    mass (ObstacleMass of motion's assets, optional, needs motion): the obstacles are free bodies of that mass; every impulse also
+    acts on the obstacle, and the touched free assets' rows of motion.asset_state are written back (agx_hp2_contact_dynamic)."""
     E = robot_state.shape[0]
     dev = robot_state.device
     if dev.type != "cuda":
@@ -325,9 +354,21 @@ def contact(scene: Optional[RayScene], robot_state: torch.Tensor, params: _lib.A
             raise ValueError("moving obstacles need a scene")
         if (motion.E, motion.K) != (scene.E, scene.K) or motion.device != dev:
             raise ValueError("motion must map this scene's [E,K] objects, on the scene's device")
+    if mass is not None:
+        if not isinstance(mass, ObstacleMass):
+            raise ValueError("mass must be an ObstacleMass")
+        if motion is None:
+            raise ValueError("dynamic obstacles need motion (their asset rows)")
+        if (mass.E, mass.A) != tuple(motion.asset_state.shape[:2]) or mass.device != dev:
+            raise ValueError("mass must have one row per motion asset [E,A], on the scene's device")
     lib = _lib.load()
     co = C.c_void_p(contact_obj.data_ptr()) if contact_obj is not None else None
     stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+    if mass is not None:
+        _lib.check(lib.agx_hp2_contact_dynamic(C.byref(scene.c), E, C.byref(params), C.byref(motion.c), C.c_void_p(mass.table.data_ptr()),
+                                               C.c_void_p(robot_state.data_ptr()), robot_state.stride(0), C.c_void_p(force.data_ptr()),
+                                               C.c_void_p(crashes.data_ptr()), co, stream), "agx_hp2_contact_dynamic")
+        return
     if motion is not None:
         _lib.check(lib.agx_hp2_contact_moving(C.byref(scene.c), E, C.byref(params), C.byref(motion.c), C.c_void_p(robot_state.data_ptr()),
                                               robot_state.stride(0), C.c_void_p(force.data_ptr()), C.c_void_p(crashes.data_ptr()), co,

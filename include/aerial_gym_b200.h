@@ -173,7 +173,7 @@ const char* agx_last_error(void);
 /* sizeof() of the ABI structs as compiled into the library (binding self-check):
  * which = 0 AgxHp1Config, 1 AgxHp1Buffers, 2 AgxHp1ResetDraws, 3 AgxHp2Scene, 4 AgxHp2Sensor,
  * 5 AgxNavRewardParams, 6 AgxImuConfig, 7 AgxLidarNavRewardParams, 8 AgxHp2Noise, 9 AgxE2ERewardParams, 10 AgxObsGatherPush,
- * 11 AgxContactParams, 12 AgxContactMotion */
+ * 11 AgxContactParams, 12 AgxContactMotion, 13 AgxObstacleMass */
 uint64_t agx_sizeof(int which);
 
 /* Host buffers the kernels can address directly (pinned, portable, mapped: cudaHostAlloc).
@@ -572,6 +572,26 @@ typedef struct AgxContactMotion {
 int agx_hp2_contact_moving(const AgxHp2Scene* scene, int num_envs, const AgxContactParams* params, const AgxContactMotion* motion,
                            float* root_state, int root_state_stride, float* contact_force, uint8_t* crashes, int32_t* contact_obj,
                            void* stream);
+
+/* Dynamic obstacles (DESIGN.md "Contact mode", "Dynamic obstacles"): every obstacle asset is one free rigid body of finite mass.
+ * The solve above acts on two bodies per contact: the relative velocity is v_robot(p) - (v_a + w_a x (p - x_a)), the inverse
+ * effective mass along d adds 1/m_a + (s x d) . I_a,w^-1 (s x d) with s = p - c_a, c_a = x_a + R_a com_a, I_a,w^-1 = R_a I_a^-1 R_a^T,
+ * and each impulse dP goes +dP to the robot, -dP to the asset.  The ground plane keeps infinite mass.  Afterwards each touched asset
+ * with a non-zero inverse mass or inertia gets its row written: the new twist (still the velocity of the asset's origin) and
+ * x_a += dt dv_a, q_a = normalize(dq(dw_a dt) (x) q_a), dq(a) = (a / 2, 1).  An asset whose entry is all zero stays kinematic: the
+ * arithmetic for it is agx_hp2_contact_moving's and its row is not written. */
+typedef struct AgxObstacleMass {
+    float inv_mass;             /* 1 / m, >= 0 */
+    float com[3];               /* centre of mass, asset frame */
+    float inertia_inv[9];       /* inverse inertia about the COM, asset-frame axes, row-major */
+} AgxObstacleMass;
+
+/* As agx_hp2_contact_moving, with the same arguments and checks, plus `mass` [E, motion->num_assets] (non-NULL).  The asset rows
+ * of motion->asset_state are read AND written: the caller passes a writable buffer.  One thread per env writes only its env's
+ * rows. */
+int agx_hp2_contact_dynamic(const AgxHp2Scene* scene, int num_envs, const AgxContactParams* params, const AgxContactMotion* motion,
+                            const AgxObstacleMass* mass, float* root_state, int root_state_stride, float* contact_force,
+                            uint8_t* crashes, int32_t* contact_obj, void* stream);
 
 
 /* ======================================================================================
