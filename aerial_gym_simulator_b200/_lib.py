@@ -151,6 +151,11 @@ class AgxObstacleMass(C.Structure):
     _fields_ = [("inv_mass", f32), ("com", f32 * 3), ("inertia_inv", f32 * 9)]
 
 
+class AgxObstacleHull(C.Structure):
+    _fields_ = [("vertices", C.c_void_p), ("file_offset", C.c_void_p), ("file_reach", C.c_void_p), ("asset_file", C.c_void_p),
+                ("num_files", C.c_int32)]
+
+
 SENSOR_CAMERA, SENSOR_LIDAR, SENSOR_STEREO_CAMERA, SENSOR_NORMAL_FACEID_CAMERA, SENSOR_NORMAL_FACEID_LIDAR = 0, 1, 2, 3, 4
 
 
@@ -228,6 +233,8 @@ def load():
                                    C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
         "agx_hp2_contact_dynamic": [C.POINTER(AgxHp2Scene), C.c_int, C.POINTER(AgxContactParams), C.POINTER(AgxContactMotion), C.c_void_p,
                                     C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
+        "agx_obstacle_ground_contact": [C.c_int, C.c_int, C.POINTER(AgxContactParams), C.c_void_p, C.c_int, C.c_void_p,
+                                        C.POINTER(AgxObstacleHull), C.c_void_p],
     }.items():
         try:
             fn = getattr(lib, name)
@@ -243,7 +250,8 @@ def load():
     if lib.agx_sizeof(5) != C.sizeof(AgxNavRewardParams) or lib.agx_sizeof(6) != C.sizeof(AgxImuConfig) \
             or lib.agx_sizeof(7) != C.sizeof(AgxLidarNavRewardParams) or lib.agx_sizeof(8) != C.sizeof(AgxHp2Noise) \
             or lib.agx_sizeof(9) != C.sizeof(AgxE2ERewardParams) or lib.agx_sizeof(11) != C.sizeof(AgxContactParams) \
-            or lib.agx_sizeof(12) != C.sizeof(AgxContactMotion) or lib.agx_sizeof(13) != C.sizeof(AgxObstacleMass):
+            or lib.agx_sizeof(12) != C.sizeof(AgxContactMotion) or lib.agx_sizeof(13) != C.sizeof(AgxObstacleMass) \
+            or lib.agx_sizeof(14) != C.sizeof(AgxObstacleHull):
         raise AgxError("aux ABI struct size mismatch between _lib.py and libaerial_gym_b200.so")
     if lib.agx_sizeof(0) != C.sizeof(AgxHp1Config) or lib.agx_sizeof(1) != C.sizeof(AgxHp1Buffers) \
             or lib.agx_sizeof(2) != C.sizeof(AgxHp1ResetDraws) or lib.agx_sizeof(10) != C.sizeof(AgxObsGatherPush):

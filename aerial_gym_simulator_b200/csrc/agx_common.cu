@@ -63,6 +63,7 @@ uint64_t agx_sizeof(int which) {
         case 11: return sizeof(AgxContactParams);
         case 12: return sizeof(AgxContactMotion);
         case 13: return sizeof(AgxObstacleMass);
+        case 14: return sizeof(AgxObstacleHull);
 #endif
         default: return 0;
     }

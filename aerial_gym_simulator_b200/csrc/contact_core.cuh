@@ -394,4 +394,88 @@ AGX_DEV void contact_env_dynamic(const AgxContactParams& P, float* rs, const Con
         if (B[b].free) contact_body_store(B[b], rows[b], P.dt);
 }
 
+// ---- Ground contact of free obstacles (agx_obstacle_ground_contact): one asset row against the plane z = 0 through the nv vertices
+// verts [nv,3] (asset frame) of its geometry, reach >= their largest distance from the asset origin.  Contacts: every vertex below
+// contact_offset, normal +z, depth -z, the AGX_CONTACT_MAX deepest kept (contact_insert on the key z: ties to the lower vertex index).
+// Solve: contact_solve_dynamic's per-contact step with the body alone against the ground at rest (infinite mass), then
+// contact_body_store.  Rows without a kept contact and kinematic rows are not written.  kept (may be NULL): the kept vertex
+// indices, deepest first.  Returns the number kept (0 for a row skipped by the reach test or kinematic).
+AGX_DEV int obstacle_ground_row(const AgxContactParams& P, float* row, const AgxObstacleMass& m, const float* verts, int nv, float reach,
+                                int* kept) {
+    if (row[2] - reach > P.contact_offset) return 0;
+    ContactBody B;
+    contact_body_load(B, row, m);
+    if (!B.free) return 0;
+    float R[9];
+    cquat_R(B.q, R);
+    ContactPt c[AGX_CONTACT_MAX];
+    float key[AGX_CONTACT_MAX];
+    int id[AGX_CONTACT_MAX];
+    int n = 0;
+    for (int j = 0; j < nv; ++j) {
+        float rv[3];
+        cmatvec(R, verts + 3 * j, rv);
+        const float z = B.x[2] + rv[2];
+        if (!(z < P.contact_offset)) continue;
+        const ContactPt pt{{B.x[0] + rv[0], B.x[1] + rv[1], z}, {0.0f, 0.0f, 1.0f}, -z};
+        n = contact_insert(c, key, id, n, pt, z, j);
+    }
+    if (kept)
+        for (int i = 0; i < n; ++i) kept[i] = id[i];
+    if (n == 0) return 0;
+    float ra[AGX_CONTACT_MAX][3], sa[AGX_CONTACT_MAX][3];
+    float kn[AGX_CONTACT_MAX], bias[AGX_CONTACT_MAX], ln[AGX_CONTACT_MAX], lt[AGX_CONTACT_MAX][3];
+    for (int i = 0; i < n; ++i) {
+        for (int k = 0; k < 3; ++k) {
+            ra[i][k] = c[i].p[k] - B.x[k];
+            sa[i][k] = c[i].p[k] - B.c[k];
+            lt[i][k] = 0.0f;
+        }
+        kn[i] = ckeff(sa[i], c[i].n, B.inv_m, B.Iw);
+        bias[i] = fminf(fmaxf(c[i].depth - P.rest_offset, 0.0f) / P.dt, P.max_depenetration_velocity);
+        ln[i] = 0.0f;
+    }
+    for (int it = 0; it < P.iterations; ++it) {
+        for (int i = 0; i < n; ++i) {
+            const float* nn = c[i].n;
+            float vr[3], dP[3];
+            // normal: accumulated impulse >= 0, target separating velocity bias
+            cvel(B.v, B.w, ra[i], vr);
+            float dl = (bias[i] - cdot(nn, vr)) / kn[i];
+            const float l1 = fmaxf(ln[i] + dl, 0.0f);
+            dl = l1 - ln[i];
+            ln[i] = l1;
+            for (int k = 0; k < 3; ++k) dP[k] = nn[k] * dl;
+            cbody_apply(dP, sa[i], B);
+            // friction: drive the tangential velocity at p to 0, accumulated impulse inside the circle mu * ln
+            cvel(B.v, B.w, ra[i], vr);
+            const float vn = cdot(nn, vr);
+            float vt[3], l2[3];
+            for (int k = 0; k < 3; ++k) {
+                vt[k] = vr[k] - nn[k] * vn;
+                l2[k] = lt[i][k];
+            }
+            const float s = sqrtf(cdot(vt, vt));
+            if (s > 0.0f) {
+                float t[3];
+                for (int k = 0; k < 3; ++k) t[k] = vt[k] / s;
+                const float dt_ = s / ckeff(sa[i], t, B.inv_m, B.Iw);
+                for (int k = 0; k < 3; ++k) l2[k] = l2[k] - t[k] * dt_;
+            }
+            const float mag = sqrtf(cdot(l2, l2)), lim = P.friction * ln[i];
+            if (mag > lim) {
+                const float f = lim / mag;
+                for (int k = 0; k < 3; ++k) l2[k] = l2[k] * f;
+            }
+            for (int k = 0; k < 3; ++k) {
+                dP[k] = l2[k] - lt[i][k];
+                lt[i][k] = l2[k];
+            }
+            cbody_apply(dP, sa[i], B);
+        }
+    }
+    contact_body_store(B, row, P.dt);
+    return n;
+}
+
 }  // namespace agx

@@ -27,6 +27,10 @@ Differences that are deliberate and documented (DESIGN.md):
         opposite, to the obstacle, and writes the pushed obstacles' twist and a first-order position correction to their rows.
         Every sub-step advances the obstacles, in steps without env_actions with their own damped velocity, so a knocked obstacle
         drifts; the scene is re-posed once more after the last sub-step; reset_idx zeroes the reset envs' obstacle velocities.
+      - ... and args['contact_obstacle_ground'] = True (needs create_ground_plane): the free obstacles also meet the ground plane.
+        Each sub-step, right after the obstacles advance, agx_obstacle_ground_contact stops every obstacle whose geometry's vertices
+        are below the plane (one-body solve against the ground, the same write-back), before the scene is re-posed and the robot
+        moves.  Obstacle-obstacle contact is not modelled.
 """
 from __future__ import annotations
 
@@ -43,8 +47,9 @@ from .. import _lib
 from .. import robots  # noqa: F401  (registers robots + controllers)
 from .. import urdf
 from ..hp1 import Hp1Engine
-from ..hp2 import ContactMotion, ObstacleMass, RayScene, RaySensor
+from ..hp2 import ContactMotion, ObstacleHull, ObstacleMass, RayScene, RaySensor
 from ..hp2 import contact as hp2_contact
+from ..hp2 import obstacle_ground_contact
 from ..registry._core import env_config_registry, robot_registry, sim_config_registry
 
 
@@ -70,6 +75,13 @@ def _obstacle_mass_row(model, path):
     if not np.linalg.matrix_rank(J) == 3:
         raise ValueError(f"{path}: the composite inertia of a free obstacle asset must be invertible")
     return ObstacleMass.row(m, com, J)
+
+
+def _hull_vertices(parts):
+    """the distinct vertices of an asset's scene parts (urdf.visual_parts, asset frame), in order of first appearance"""
+    v = np.concatenate([t.reshape(-1, 3) for _, _, t, _ in parts]) if parts else np.zeros((0, 3), np.float32)
+    _, first = np.unique(v, axis=0, return_index=True)
+    return v[np.sort(first)]
 
 
 def _quat_rotate_inverse(q, v):
@@ -146,6 +158,14 @@ class EnvManager:
         if dynamic and not moving:
             raise ValueError("args['contact_dynamic_obstacles'] needs args['contact_moving_obstacles'] = True")
         self.contact_dynamic_obstacles = dynamic
+        ground = self.env_args.get("contact_obstacle_ground", False)
+        if not isinstance(ground, bool):
+            raise ValueError("args['contact_obstacle_ground'] must be a bool")
+        if ground and not dynamic:
+            raise ValueError("args['contact_obstacle_ground'] needs args['contact_dynamic_obstacles'] = True")
+        if ground and not bool(getattr(self.cfg.env, "create_ground_plane", False)):
+            raise ValueError("args['contact_obstacle_ground'] needs an env with create_ground_plane")
+        self.contact_obstacle_ground = ground
         self.global_tensor_dict = {}
         self.step_counter = 0
         self._graphs, self._dist_ctr_dev = {}, None
@@ -232,6 +252,10 @@ class EnvManager:
         self._obstacle_mass = None
         if self._contact_motion is not None and self.contact_dynamic_obstacles:
             self._obstacle_mass = ObstacleMass(self._asset_mass.to(dev))
+        # the obstacle-ground solve: every asset's vertices (table built in _build_obstacles)
+        self._obstacle_hull = None
+        if self._obstacle_mass is not None and self.contact_obstacle_ground:
+            self._obstacle_hull = ObstacleHull.from_files(self._hull_files, self._asset_file, dev)
 
     # ---- obstacles: AssetLoader.select_assets_for_sim + WarpEnv (asset_loader.py:148-194, warp_env_manager.py)
     def _select_assets(self):
@@ -299,6 +323,9 @@ class EnvManager:
         # dynamic obstacles: one mass-table row per distinct URDF (inverse mass, COM, inverse inertia: AgxObstacleMass)
         dynamic = self.contact_dynamic_obstacles
         mass_of, asset_mass = {}, (np.zeros((N, A, 13), np.float32) if dynamic else None)
+        # obstacle-ground contact: the vertices of each distinct URDF's scene parts, and each asset's file
+        ground = self.contact_obstacle_ground
+        file_of, hull_files, asset_file = {}, [], (np.zeros((N, A), np.int32) if ground else None)
         for e in range(N):
             for a, (params, path) in enumerate(per_env[e]):
                 lo[e, a], hi[e, a] = params.min_state_ratio, params.max_state_ratio
@@ -310,7 +337,11 @@ class EnvManager:
                     if dynamic:
                         mass_of[path] = _obstacle_mass_row(model, path)
                     ids = []
-                    for _, link_index, tris, obb in urdf.visual_parts(model, params.use_collision_mesh_instead_of_visual):
+                    parts = urdf.visual_parts(model, params.use_collision_mesh_instead_of_visual)
+                    if ground:
+                        file_of[path] = len(hull_files)
+                        hull_files.append(_hull_vertices(parts))
+                    for _, link_index, tris, obb in parts:
                         if obb is None:
                             ids.append(-1 - len(meshes))
                             meshes.append(tris)
@@ -323,8 +354,12 @@ class EnvManager:
                     boxes_of[path] = ids
                 if dynamic:
                     asset_mass[e, a] = mass_of[path]
+                if ground:
+                    asset_file[e, a] = file_of[path]
         if dynamic:
             self._asset_mass = torch.from_numpy(asset_mass)
+        if ground:
+            self._hull_files, self._asset_file = hull_files, asset_file
         gtd["asset_min_state_ratio"].copy_(torch.from_numpy(lo))
         gtd["asset_max_state_ratio"].copy_(torch.from_numpy(hi))
         if not self.use_warp:
@@ -561,7 +596,8 @@ class EnvManager:
         10 sub-steps per env step (config/env_config/env_with_obstacles.py:29-30): ~30 launches become one.
         Dynamic obstacles (args['contact_dynamic_obstacles'], fixed for the manager, so (n, moving) keys the graph): every sub-step
         advances the obstacles, with the env_actions twist when moving and with their own velocity otherwise, the solve writes the
-        obstacles it pushes, and the scene is re-posed once more after the last sub-step."""
+        obstacles it pushes, and the scene is re-posed once more after the last sub-step.  With args['contact_obstacle_ground'] (also
+        fixed for the manager) each sub-step's obstacle advance is followed by the obstacle-ground solve."""
         g = self._graphs.get((n, moving))
         if g is not None:
             return g
@@ -708,9 +744,12 @@ class EnvManager:
 
     def _move_obstacles_one_substep(self, with_twist=True):
         """contact with moving obstacles: one sub-step of the obstacles (the advance keeps its state in float32, so n of these add
-        up bit for bit to one n-sub-step advance) and the scene re-posed where they now are.  with_twist False (dynamic obstacles in
-        a step without env_actions): each obstacle keeps its own damped velocity."""
+        up bit for bit to one n-sub-step advance), with args['contact_obstacle_ground'] the obstacle-ground solve, and the scene
+        re-posed where they now are.  with_twist False (dynamic obstacles in a step without env_actions): each obstacle keeps its own
+        damped velocity."""
         self._advance_obstacles(self.global_tensor_dict["env_actions"] if with_twist else None, 1)
+        if self._obstacle_hull is not None:  # obstacle-ground contact: the robot's contact search sees the corrected obstacles
+            obstacle_ground_contact(self.contact_params, self._contact_motion, self._obstacle_mass, self._obstacle_hull)
         self._repose_scene()
 
     def compute_observations(self, moving_obstacles=False):

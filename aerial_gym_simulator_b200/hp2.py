@@ -322,6 +322,81 @@ class ObstacleMass:
                                np.linalg.inv(np.asarray(inertia, np.float64).reshape(3, 3)).reshape(9)]).astype(np.float32)
 
 
+class ObstacleHull:
+    """The vertex table of the obstacle–ground contact (agx_obstacle_ground_contact), one AgxObstacleHull.
+    vertices: float32 [V,3], the asset-frame vertices of every file, file after file; file_offset: integer [F+1], file f's vertices
+    are vertices[file_offset[f]:file_offset[f+1]]; file_reach: float32 [F], each >= the largest distance of the file's vertices from
+    the asset origin; asset_file: integer [E,A], the file of each (env, asset).  Checked here once (one host read): finite values,
+    offsets from 0, non-decreasing and ending at V, every asset_file in [0, F).  Kept as contiguous copies on vertices' device
+    (int32 indices)."""
+
+    def __init__(self, vertices: torch.Tensor, file_offset: torch.Tensor, file_reach: torch.Tensor, asset_file: torch.Tensor):
+        for name, x, fp in (("vertices", vertices, True), ("file_offset", file_offset, False), ("file_reach", file_reach, True),
+                            ("asset_file", asset_file, False)):
+            if not isinstance(x, torch.Tensor) or x.is_floating_point() != fp or x.dtype == torch.bool or x.is_complex():
+                raise ValueError(f"{name} must be a{' floating-point' if fp else 'n integer'} tensor")
+        dev = vertices.device
+        v, off, reach, af = (x.to(device=dev, dtype=dt).contiguous() for x, dt in (
+            (vertices, torch.float32), (file_offset, torch.int32), (file_reach, torch.float32), (asset_file, torch.int32)))
+        if v.dim() != 2 or v.shape[1] != 3:
+            raise ValueError("vertices must be [V,3]")
+        if reach.dim() != 1 or reach.shape[0] < 1 or off.shape != (reach.shape[0] + 1,):
+            raise ValueError("file_reach must be [F>=1] and file_offset [F+1]")
+        if af.dim() != 2 or af.shape[1] < 1:
+            raise ValueError("asset_file must be [E,A>=1]")
+        F, V = reach.shape[0], v.shape[0]
+        checks = torch.stack([torch.isfinite(v).all(), torch.isfinite(reach).all(), (reach >= 0).all(), off[0] == 0, off[-1] == V,
+                              (off[1:] >= off[:-1]).all(), (af >= 0).all(), (af < F).all()]).cpu()
+        msgs = ("vertices must be finite", "file_reach must be finite", "file_reach must be >= 0", "file_offset must start at 0",
+                f"file_offset must end at V = {V}", "file_offset must be non-decreasing", f"asset_file values must be in [0, {F})",
+                f"asset_file values must be in [0, {F})")
+        for ok, msg in zip(checks.tolist(), msgs):
+            if not ok:
+                raise ValueError(msg)
+        self.vertices, self.file_offset, self.file_reach, self.asset_file = v, off, reach, af
+        self.E, self.A, self.F, self.device = af.shape[0], af.shape[1], F, v.device
+        self.c = _lib.AgxObstacleHull(vertices=v.data_ptr(), file_offset=off.data_ptr(), file_reach=reach.data_ptr(),
+                                      asset_file=af.data_ptr(), num_files=F)
+
+    @classmethod
+    def from_files(cls, file_vertices, asset_file, device):
+        """from a list of per-file vertex arrays ([n,3], asset frame) and the [E,A] file index; each file's reach is the largest
+        distance of its vertices from the origin, rounded up to the next float32"""
+        vs = [np.asarray(x, np.float32).reshape(-1, 3) for x in file_vertices]
+        reach = np.array([np.sqrt((x.astype(np.float64) ** 2).sum(1)).max() if len(x) else 0.0 for x in vs], np.float32)
+        reach = np.nextafter(reach, np.float32(np.inf))
+        off = np.concatenate([[0], np.cumsum([len(x) for x in vs])]).astype(np.int32)
+        v = np.concatenate(vs) if vs else np.zeros((0, 3), np.float32)
+        return cls(*(torch.from_numpy(np.ascontiguousarray(x)).to(device) for x in (v, off, reach, np.asarray(asset_file))))
+
+
+def obstacle_ground_contact(params: _lib.AgxContactParams, motion: ContactMotion, mass: ObstacleMass, hull: ObstacleHull):
+    """agx_obstacle_ground_contact: every free obstacle asset of motion.asset_state [E,A,>=13] against the ground plane z = 0 through
+    the vertices of its file in hull; the rows with a kept contact get their new twist and position correction in place.  Of params
+    only contact_offset, rest_offset, dt, friction, max_depenetration_velocity and iterations are read."""
+    if not isinstance(params, _lib.AgxContactParams):
+        raise ValueError("params must be an AgxContactParams")
+    if not isinstance(motion, ContactMotion):
+        raise ValueError("motion must be a ContactMotion")
+    if not isinstance(mass, ObstacleMass):
+        raise ValueError("mass must be an ObstacleMass")
+    if not isinstance(hull, ObstacleHull):
+        raise ValueError("hull must be an ObstacleHull")
+    st = motion.asset_state
+    dev = st.device
+    E, A = st.shape[0], st.shape[1]
+    if (mass.E, mass.A) != (E, A) or mass.device != dev:
+        raise ValueError("mass must have one row per motion asset [E,A], on the asset rows' device")
+    if (hull.E, hull.A) != (E, A) or hull.device != dev:
+        raise ValueError("hull must have one file index per motion asset [E,A], on the asset rows' device")
+    if dev.type != "cuda":
+        raise _lib.AgxError("obstacle_ground_contact needs a CUDA device: there is no CPU path")
+    _lib.check(_lib.load().agx_obstacle_ground_contact(E, A, C.byref(params), C.c_void_p(st.data_ptr()), st.stride(1),
+                                                       C.c_void_p(mass.table.data_ptr()), C.byref(hull.c),
+                                                       C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+               "agx_obstacle_ground_contact")
+
+
 def contact(scene: Optional[RayScene], robot_state: torch.Tensor, params: _lib.AgxContactParams, force: torch.Tensor,
             crashes: torch.Tensor, contact_obj: Optional[torch.Tensor] = None, motion: Optional[ContactMotion] = None,
             mass: Optional[ObstacleMass] = None):

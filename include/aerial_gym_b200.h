@@ -173,7 +173,7 @@ const char* agx_last_error(void);
 /* sizeof() of the ABI structs as compiled into the library (binding self-check):
  * which = 0 AgxHp1Config, 1 AgxHp1Buffers, 2 AgxHp1ResetDraws, 3 AgxHp2Scene, 4 AgxHp2Sensor,
  * 5 AgxNavRewardParams, 6 AgxImuConfig, 7 AgxLidarNavRewardParams, 8 AgxHp2Noise, 9 AgxE2ERewardParams, 10 AgxObsGatherPush,
- * 11 AgxContactParams, 12 AgxContactMotion, 13 AgxObstacleMass */
+ * 11 AgxContactParams, 12 AgxContactMotion, 13 AgxObstacleMass, 14 AgxObstacleHull */
 uint64_t agx_sizeof(int which);
 
 /* Host buffers the kernels can address directly (pinned, portable, mapped: cudaHostAlloc).
@@ -592,6 +592,32 @@ typedef struct AgxObstacleMass {
 int agx_hp2_contact_dynamic(const AgxHp2Scene* scene, int num_envs, const AgxContactParams* params, const AgxContactMotion* motion,
                             const AgxObstacleMass* mass, float* root_state, int root_state_stride, float* contact_force,
                             uint8_t* crashes, int32_t* contact_obj, void* stream);
+
+/* Ground contact of free obstacles (DESIGN.md "Contact mode", "Ground contact of free obstacles"): each free obstacle asset against
+ * the plane z = 0 through the vertices of its scene geometry.  Per file f, vertices[file_offset[f] .. file_offset[f+1]) are its
+ * vertices in the asset frame and file_reach[f] bounds their distance from the asset origin; asset a of env e uses file
+ * asset_file[e,a].  Every value of asset_file is in [0, num_files) and the offsets are non-decreasing: the caller checks this when
+ * it builds the table, the kernel reads without a bounds check. */
+typedef struct AgxObstacleHull {
+    const float* vertices;      /* [V,3] asset frame, file after file */
+    const int32_t* file_offset; /* [F+1], file_offset[0] = 0, file_offset[F] = V */
+    const float* file_reach;    /* [F] >= the largest |vertex| of the file */
+    const int32_t* asset_file;  /* [E,A] */
+    int32_t num_files;          /* F >= 1 */
+} AgxObstacleHull;
+
+/* One thread per (env, asset) row of asset_state [E,A,asset_stride] (rows x y z qx qy qz qw vx vy vz wx wy wz, read AND written).
+ * A row with z - reach > contact_offset has no contact and is left after that one compare; so is a kinematic row (all-zero mass
+ * entry).  Otherwise every vertex with world height z < contact_offset is a candidate contact at p = the vertex, normal +z, depth
+ * -z; the AGX_CONTACT_MAX deepest are kept (ties to the lower vertex index), deepest first, which is the solve order.  The solve is
+ * agx_hp2_contact_dynamic's per-contact step for one body against an infinite-mass ground at rest, `iterations` passes: relative
+ * velocity v_a + w_a x (p - x_a), inverse effective mass 1/m_a + (s x d) . I_a,w^-1 (s x d) with s = p - c_a, the normal row's target
+ * min(max(depth - rest_offset, 0) / dt, max_depenetration_velocity), Coulomb friction in the circle |lambda_t| <= friction lambda_n.
+ * A row with a kept contact gets agx_hp2_contact_dynamic's write-back (new twist, x += dt dv, q = normalize(dq(dw dt) (x) q)).
+ * Of params only contact_offset, rest_offset, dt, friction, max_depenetration_velocity and iterations are read; the robot's fields
+ * (radius, mass, inertia_inv, com, force_threshold, ground_plane) are ignored.  mass [E,A] as agx_hp2_contact_dynamic's. */
+int agx_obstacle_ground_contact(int num_envs, int num_assets, const AgxContactParams* params, float* asset_state, int asset_stride,
+                                const AgxObstacleMass* mass, const AgxObstacleHull* hull, void* stream);
 
 
 /* ======================================================================================
