@@ -14,8 +14,7 @@ LIB = os.path.join(PKG, "libaerial_gym_b200.so")
 UNITS = [
     ("agx_common.cu", []),
     # hp1: 2-ulp division / sqrt (no slow-path branches): the step is a long dependent chain per warp, every instruction counts
-    # AGX_HP1_NOINLINE_TRIG: one shared out-of-line sincosf instead of seven inlined copies (same function, same bits)
-    ("hp1.cu", ["-prec-div=false", "-prec-sqrt=false", "-DAGX_HP1_NOINLINE_TRIG"]),  # AGX_FAST_TRIG: 3x parity error -> off
+    ("hp1.cu", ["-prec-div=false", "-prec-sqrt=false"]),  # AGX_FAST_TRIG: 3x parity error -> off
     ("hp1_aux.cu", []),
     ("lidar_nav.cu", []),
     # device-RNG units: no FMA contraction, so "lo + (hi - lo) u" and the noise model round like their numpy oracles

@@ -18,12 +18,10 @@ namespace agx {
 
 // sin/cos of an angle in [-2pi, 2pi].  AGX_FAST_TRIG: MUFU.SIN/COS (__sincosf, abs error <= 2^-21.4
 // on [-pi, pi], CUDA C Programming Guide table 9) instead of the ~40-instruction libdevice path.
+// Always inline: one shared out-of-line copy sends every value live across its calls through the stack, and in the HP1 step kernel
+// that put local-memory traffic inside the physics sub-step loop (DESIGN 6).
 #ifdef AGX_FAST_TRIG
 AGX_DEV void sincos_(float x, float* s, float* c) { __sincosf(x, s, c); }
-#elif defined(AGX_HP1_NOINLINE_TRIG) && !defined(AGX_HOST_SHADOW)
-// round-2 experiment (tools/build_variant.py): ONE copy of the accurate sincosf per kernel instead of one per call site
-__device__ __noinline__ void sincos_shared_(float x, float* s, float* c) { sincosf(x, s, c); }
-AGX_DEV void sincos_(float x, float* s, float* c) { sincos_shared_(x, s, c); }
 #else
 AGX_DEV void sincos_(float x, float* s, float* c) { sincosf(x, s, c); }
 #endif

@@ -7,7 +7,6 @@ All translation units of aerial_gym_simulator_b200/_build.py are compiled (same 
 Round-2 candidates for the latency / instruction-fetch bound HP1 step (DESIGN 11; numerically identical to the default build --
 the CPU shadow tests run the same text with the same macro: AGX_SHADOW_FLAGS="-DAGX_HP1_ROLL_MOTORS" python -m pytest tests -m "not gpu"):
     --hp1 "-DAGX_HP1_ROLL_MOTORS"     motor / allocation loops rolled (#pragma unroll 1): ~4x less straight-line code to fetch
-    --hp1 "-DAGX_HP1_NOINLINE_TRIG"   one shared copy of sincosf instead of seven inlined ones
     --hp1 "-maxrregcount=96"          (or __launch_bounds__ experiments)"""
 import os
 import shlex
