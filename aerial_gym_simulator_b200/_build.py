@@ -16,6 +16,7 @@ UNITS = [
     # hp1: 2-ulp division / sqrt (no slow-path branches): the step is a long dependent chain per warp, every instruction counts
     ("hp1.cu", ["-prec-div=false", "-prec-sqrt=false"]),  # AGX_FAST_TRIG: 3x parity error -> off
     ("hp1_aux.cu", []),
+    ("articulated.cu", []),
     ("lidar_nav.cu", []),
     # device-RNG units: no FMA contraction, so "lo + (hi - lo) u" and the noise model round like their numpy oracles
     ("sensor_noise.cu", ["-fmad=false"]),

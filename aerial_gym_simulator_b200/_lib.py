@@ -156,6 +156,19 @@ class AgxObstacleHull(C.Structure):
                 ("num_files", C.c_int32)]
 
 
+ART_MAX_BODIES = 16  # AGX_ART_MAX_BODIES
+
+
+class AgxArticulation(C.Structure):
+    B, M = ART_MAX_BODIES, AGX_MAX_MOTORS
+    _fields_ = [("num_bodies", C.c_int32), ("num_dofs", C.c_int32), ("parent", C.c_int32 * B),
+                ("joint_R", (f32 * 9) * B), ("joint_p", (f32 * 3) * B), ("axis", (f32 * 3) * B), ("mass", f32 * B),
+                ("com", (f32 * 3) * B), ("inertia", (f32 * 9) * B), ("lower", f32 * B), ("upper", f32 * B), ("limited", C.c_int32 * B),
+                ("stiffness", f32 * B), ("damping", f32 * B), ("motor_body", C.c_int32 * M), ("motor_R", (f32 * 9) * M),
+                ("motor_p", (f32 * 3) * M), ("motor_torque", f32 * M), ("dof_state", fp), ("dof_position_setpoint", fp),
+                ("dof_velocity_setpoint", fp)]
+
+
 SENSOR_CAMERA, SENSOR_LIDAR, SENSOR_STEREO_CAMERA, SENSOR_NORMAL_FACEID_CAMERA, SENSOR_NORMAL_FACEID_LIDAR = 0, 1, 2, 3, 4
 
 
@@ -192,6 +205,7 @@ def load():
         "agx_hp1_position_task_step": [C.POINTER(AgxHp1Config), C.POINTER(AgxHp1Buffers), C.c_void_p],
         "agx_hp1_position_task_step_profiled": [C.POINTER(AgxHp1Config), C.POINTER(AgxHp1Buffers), C.c_void_p,
                                                 C.c_void_p],
+        "agx_hp1_articulated_step": [C.POINTER(AgxHp1Config), C.POINTER(AgxHp1Buffers), C.POINTER(AgxArticulation), C.c_void_p],
         "agx_hp1_reset": [C.POINTER(AgxHp1Config), C.POINTER(AgxHp1Buffers), C.c_void_p,
                           C.POINTER(AgxHp1ResetDraws), C.c_void_p],
         "agx_hp1_refresh": [C.POINTER(AgxHp1Config), C.POINTER(AgxHp1Buffers), C.c_int, C.c_void_p],
@@ -254,7 +268,8 @@ def load():
             or lib.agx_sizeof(14) != C.sizeof(AgxObstacleHull):
         raise AgxError("aux ABI struct size mismatch between _lib.py and libaerial_gym_b200.so")
     if lib.agx_sizeof(0) != C.sizeof(AgxHp1Config) or lib.agx_sizeof(1) != C.sizeof(AgxHp1Buffers) \
-            or lib.agx_sizeof(2) != C.sizeof(AgxHp1ResetDraws) or lib.agx_sizeof(10) != C.sizeof(AgxObsGatherPush):
+            or lib.agx_sizeof(2) != C.sizeof(AgxHp1ResetDraws) or lib.agx_sizeof(10) != C.sizeof(AgxObsGatherPush) \
+            or lib.agx_sizeof(15) != C.sizeof(AgxArticulation):
         raise AgxError("ABI struct size mismatch between _lib.py and libaerial_gym_b200.so")
     _lib = lib
     return lib

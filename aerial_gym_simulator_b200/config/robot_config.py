@@ -428,7 +428,7 @@ class BaseROVCfg(BaseOctarotorCfg):
 
 class MorphyStiffCfg(BaseQuadCfg):
     """config/robot_config/morphy_stiff_config.py: the Morphy airframe with its arm joints welded (every joint of morphy_stiff.urdf is
-    fixed) -- a plain rigid quadrotor; the compliant-arm Morphy itself needs joint dynamics and is out of scope"""
+    fixed) -- a plain rigid quadrotor.  MorphyCompliantCfg below frees two joints per arm."""
     class init_config:
         min_init_state = [0.0, 0.0, 0.0, 0, 0, -PI / 6, 1.0, -0.2, -0.2, -0.2, -0.2, -0.2, -0.2]
         max_init_state = [1.0, 1.0, 1.0, 0, 0, PI / 6, 1.0, 0.2, 0.2, 0.2, 0.2, 0.2, 0.2]
@@ -452,3 +452,24 @@ class MorphyStiffCfg(BaseQuadCfg):
             motor_time_constant_increasing_max = 0.03
             motor_time_constant_decreasing_min = 0.005
             motor_time_constant_decreasing_max = 0.005
+
+
+class MorphyCompliantCfg(MorphyStiffCfg):
+    """Morphy with compliant arms (ours: the reference's own morphy.urdf and config are not in this tree).  morphy_compliant.urdf is
+    morphy_stiff.urdf with two revolute joints per arm: base_link_to_connecting_link_i sweeps the arm in the base plane,
+    connecting_link_to_arm_motor_i flaps it up and down, both within +-0.6 rad.  The drive gains are OUR values, not Morphy's
+    measured ones (DESIGN.md "Articulated robots" derives them): an arm's inertia about either joint is 0.01625 kg x (0.07 m)^2 =
+    8.0e-5 kg m^2, so k = 1.0 N m / rad gives w = 112 rad/s and a hover flap deflection of ~0.05 rad, and d = 3.6e-3 N m s / rad a
+    damping ratio of 0.2."""
+    class robot_asset(MorphyStiffCfg.robot_asset):
+        file = "morphy_compliant.urdf"
+
+    class joint_config:
+        # per DOF, in the order of the merged body table (sweep_0, flap_0, sweep_1, flap_1, ...); a scalar applies to all
+        stiffness = 1.0
+        damping = 3.6e-3
+        # uniform reset ranges of the joint state (position rad, velocity rad/s)
+        min_init_dof_position = -0.1
+        max_init_dof_position = 0.1
+        min_init_dof_velocity = 0.0
+        max_init_dof_velocity = 0.0

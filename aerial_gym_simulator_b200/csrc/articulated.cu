@@ -1,0 +1,75 @@
+// Articulated multirotors: the physics-only step of agx_hp1_physics_step for a robot whose URDF tree has revolute joints
+// (DESIGN.md "Articulated robots").  The per-env arithmetic is articulated_core.cuh; this unit holds the kernel and the entry point.
+//
+// Layout: one env per thread, every per-body array of the ABA in the thread's own local memory.  The sweeps over the tree index
+// those arrays with the run-time parent table, so they cannot live in registers; a warp's 32 envs walk the same tree in lockstep,
+// so their accesses coalesce (local memory is interleaved per thread) and stay in L1 / L2.  The alternative -- one warp per env,
+// lanes over the bodies of a tree level -- would keep the scratch in registers and shuffles but leave most lanes idle on a
+// 9-body tree whose levels are 1, 4 and 4 bodies wide, and the controller / motor part of the sub-step (a third of its
+// instructions) would run on one lane.  DESIGN.md records the measured cost.
+#include <cuda_runtime.h>
+#include <stdint.h>
+
+#include "../../include/aerial_gym_b200.h"
+#include "agx_common.cuh"
+#include "articulated_core.cuh"
+
+using namespace agx;
+
+namespace {
+
+constexpr int kArtThreads = 128;
+
+template <int M, int NB>
+__global__ void __launch_bounds__(kArtThreads)
+articulated_step_kernel(const __grid_constant__ AgxHp1Config cfg, const __grid_constant__ AgxHp1Buffers buf,
+                        const __grid_constant__ AgxArticulation art) {
+    const int env = blockIdx.x * blockDim.x + threadIdx.x;
+    if (env >= cfg.num_envs) return;
+    art_env_step<M, NB>(cfg, buf, art, env);
+}
+
+int validate_articulation(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, const AgxArticulation* art) {
+    if (!cfg || !buf || !art) return agx_set_error(AGX_E_NULL, "cfg/buf/art is NULL");
+    if (cfg->num_envs < 0) return agx_set_error(AGX_E_INVALID, "num_envs < 0");
+    if (cfg->num_motors != 4 && cfg->num_motors != 8)
+        return agx_set_error(AGX_E_INVALID, "num_motors must be 4 or 8 (got %d)", cfg->num_motors);
+    if (cfg->controller < AGX_CTRL_NONE || cfg->controller > AGX_CTRL_VELOCITY_STEERING)
+        return agx_set_error(AGX_E_INVALID, "unknown controller id %d", cfg->controller);
+    const int need = (cfg->controller == AGX_CTRL_NONE) ? cfg->num_motors : (cfg->controller == AGX_CTRL_FULLY_ACTUATED ? 7 : 4);
+    if (cfg->num_actions != need)
+        return agx_set_error(AGX_E_INVALID, "controller %d needs %d action columns (got %d)", cfg->controller, need, cfg->num_actions);
+    if (cfg->physics_steps < 0) return agx_set_error(AGX_E_INVALID, "physics_steps < 0");
+    const int B = art->num_bodies;
+    if (B < 1 || B > AGX_ART_MAX_BODIES)
+        return agx_set_error(AGX_E_INVALID, "num_bodies must be in [1, %d] (got %d)", AGX_ART_MAX_BODIES, B);
+    if (art->num_dofs != B - 1) return agx_set_error(AGX_E_INVALID, "num_dofs must be num_bodies - 1");
+    for (int i = 1; i < B; ++i)
+        if (art->parent[i] < 0 || art->parent[i] >= i) return agx_set_error(AGX_E_INVALID, "parent[%d] must be in [0, %d)", i, i);
+    for (int k = 0; k < cfg->num_motors; ++k)
+        if (art->motor_body[k] < 0 || art->motor_body[k] >= B) return agx_set_error(AGX_E_INVALID, "motor_body[%d] out of range", k);
+    if (cfg->num_envs == 0) return AGX_OK;
+    if (!buf->root_state || !buf->motor_thrust || !buf->actions) return agx_set_error(AGX_E_NULL, "root_state/motor_thrust/actions is NULL");
+    if (buf->body_wrench) return agx_set_error(AGX_E_INVALID, "the articulated step does not write body_wrench: pass NULL");
+    if (B > 1 && (!art->dof_state || !art->dof_position_setpoint || !art->dof_velocity_setpoint))
+        return agx_set_error(AGX_E_NULL, "dof_state/dof_position_setpoint/dof_velocity_setpoint is NULL");
+    return AGX_OK;
+}
+
+using ArtKernel = void (*)(const AgxHp1Config, const AgxHp1Buffers, const AgxArticulation);
+// per-body scratch sized for the tree: up to 9 bodies (a quadrotor with two joints per arm) or the full 16
+ArtKernel pick_art_kernel(int M, int B) {
+    if (M == 4) return B <= 9 ? articulated_step_kernel<4, 9> : articulated_step_kernel<4, AGX_ART_MAX_BODIES>;
+    return B <= 9 ? articulated_step_kernel<8, 9> : articulated_step_kernel<8, AGX_ART_MAX_BODIES>;
+}
+
+}  // namespace
+
+extern "C" int agx_hp1_articulated_step(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, const AgxArticulation* art, void* stream) {
+    int rc = validate_articulation(cfg, buf, art);
+    if (rc) return rc;
+    if (cfg->num_envs == 0) return AGX_OK;
+    const int g = (cfg->num_envs + kArtThreads - 1) / kArtThreads;
+    pick_art_kernel(cfg->num_motors, art->num_bodies)<<<g, kArtThreads, 0, (cudaStream_t)stream>>>(*cfg, *buf, *art);
+    return agx_check_launch("articulated_step_kernel");
+}

@@ -110,7 +110,7 @@ class _SimView:
 
     def __init__(self, env):
         self._env, self.sim_config, self.num_envs = env, env.sim_config, env.num_envs
-        self.sim_has_dof, self.dof_control_mode, self.viewer, self.has_viewer = False, "none", None, False
+        self.sim_has_dof, self.dof_control_mode, self.viewer, self.has_viewer = env.articulated, "none", None, False
 
     num_assets_per_env = property(lambda self: self._env.num_obs_in_env + 1)  # :269-276, the robot is an actor too
     num_rigid_bodies_robot = property(lambda self: self._env.robot.num_bodies)
@@ -191,13 +191,32 @@ class EnvManager:
         self.num_robot_actions = self.robot.num_actions
         spec = self.robot.make_spec(self.sim_config, self.cfg)
         self.spec = spec
+        self.articulated = bool(getattr(self.robot, "articulated", False))
+        articulation = None
+        if self.articulated:
+            if self.contact_mode == "rigid":
+                raise ValueError("args['contact'] = 'rigid' is not available for an articulated robot: the contact solve gives its impulse "
+                                 "to the base alone, which is wrong for a tree of bodies")
+            if getattr(self.robot_cfg.sensor_config, "enable_imu", False):
+                raise ValueError("the IMU is not available on an articulated robot: its force input would need the joint reaction forces")
+            if bool(self.env_args.get("host_io", False)):
+                raise NotImplementedError("args['host_io'] is a feature of the fused task step, which articulated robots do not have")
+            articulation = self.robot.make_articulation()
         self.engine = Hp1Engine(
             spec, N, dev, physics_steps=1, seed=int(self.env_args.get("seed", 0)),
             env_id_offset=int(self.env_args.get("env_id_offset", 0)), device_rng_reset=(self.reset_rng == "device"),
             strict_stale_obs=bool(self.env_args.get("strict_stale_obs", True)), materialize_derived=True,
             per_env_params=self.env_args.get("per_env_params", "auto"), host_io=bool(self.env_args.get("host_io", False)),
-            debug_wrench=bool(getattr(self.robot_cfg.sensor_config, "enable_imu", False)))  # the IMU reads the net body force
+            debug_wrench=bool(getattr(self.robot_cfg.sensor_config, "enable_imu", False)),  # the IMU reads the net body force
+            **({"articulation": articulation} if articulation is not None else {}))
         eng, gtd = self.engine, self.global_tensor_dict
+        if articulation is not None:
+            # joint state (position, velocity) and the drive targets; the targets belong to the user: the env never writes them
+            gtd["dof_state_tensor"] = eng.dof_state
+            gtd["dof_position_setpoint_tensor"] = eng.dof_position_setpoint
+            gtd["dof_velocity_setpoint_tensor"] = eng.dof_velocity_setpoint
+            T = lambda v: torch.tensor(np.asarray(v, np.float32), device=dev)
+            self._dof_rng = tuple(T(r) for r in (*articulation.init_dof_pos_range, *articulation.init_dof_vel_range))
         self.robot.controller.bind_engine(eng)  # controller.K_*_tensor_current / set_controller_gains act on the engine's gains
         gtd["crashes"], gtd["truncations"] = eng.terminations, eng.truncations
         self.collision_tensor, self.truncation_tensor = eng.terminations, eng.truncations
@@ -522,6 +541,13 @@ class EnvManager:
             for k, t in saved_motors.items():
                 getattr(eng, k)[env_ids] = t[env_ids]
         self._motors_initialised = True
+        if self.articulated:
+            # joint state: uniform in the joint_config ranges, drawn full-size on the device and selected by the mask (no host sync)
+            D = eng.dof_state.shape[1]
+            u = torch.rand(N, D, 2, device=dev)
+            p0, p1, v0, v1 = self._dof_rng
+            new = torch.stack([_lerp(p0, p1, u[..., 0]), _lerp(v0, v1, u[..., 1])], dim=-1)
+            eng.dof_state.copy_(torch.where(mask.view(N, 1, 1), new, eng.dof_state))
         if self.sensor is not None and self.sensor_cfg.randomize_placement:  # warp_sensor.py:153-172
             k, S = len(env_ids), self.sensor_cfg.num_sensors
             t0, t1, e0, e1 = self._mount_rng
@@ -630,12 +656,15 @@ class EnvManager:
                     None if not dist else self._dist_ctr_dev.clone())
             force = self.global_tensor_dict["robot_contact_force_tensor"]
             keep_force = force.clone()
+            keep_dof = eng.dof_state.clone() if getattr(eng, "dof_state", None) is not None else None  # articulated robots
             if moving or dynamic:
                 ast = self.global_tensor_dict["env_asset_state_tensor"]
                 keep_obstacles = (ast.clone(), self._obj_pose.clone())
             body()
             eng.root_state.copy_(keep[0]); eng.motor_thrust.copy_(keep[1]); self.collision_tensor.copy_(keep[2])
             force.copy_(keep_force)
+            if keep_dof is not None:
+                eng.dof_state.copy_(keep_dof)
             if dist:
                 self._dist_ctr_dev.copy_(keep[3])
             if moving or dynamic:

@@ -122,6 +122,82 @@ class MultirotorSpec:
         return torch.linalg.pinv(A).double().numpy()
 
 
+@dataclass
+class ArticulationSpec:
+    """The joint layer of an articulated multirotor (DESIGN.md "Articulated robots"): the merged body table of its URDF
+    (urdf.ArticulatedBodies), the drive gains per DOF, where each motor sits, and the ranges the joint state is reset to.
+    The MultirotorSpec beside it keeps the zero-configuration mass and inertia, which is what the controller uses."""
+
+    bodies: object                     # urdf.ArticulatedBodies
+    stiffness: np.ndarray              # [D] k, N m / rad
+    damping: np.ndarray                # [D] d, N m s / rad (the URDF <dynamics damping> is added on top)
+    motor_body: np.ndarray             # [M] body of each motor's application_mask link
+    motor_R: np.ndarray                # [M,3,3] motor link frame in its body's frame
+    motor_p: np.ndarray                # [M,3]
+    motor_torque: np.ndarray           # [M] reaction torque per unit thrust about the motor z axis: -thrust_to_torque_ratio * dir
+    init_dof_pos_range: tuple = None   # ([D], [D]) uniform reset range of q; default (0, 0)
+    init_dof_vel_range: tuple = None   # ([D], [D]) of q-dot
+
+    def __post_init__(self):
+        b, D = self.bodies, self.bodies.num_dofs
+        z = np.zeros(D)
+        self.stiffness = np.broadcast_to(np.asarray(self.stiffness, np.float64), (D,)).copy()
+        self.damping = np.broadcast_to(np.asarray(self.damping, np.float64), (D,)).copy()
+        if (self.stiffness < 0).any() or (self.damping < 0).any():
+            raise ValueError("joint stiffness and damping must be >= 0")
+        rng = lambda r: (z.copy(), z.copy()) if r is None else tuple(np.broadcast_to(np.asarray(v, np.float64), (D,)).copy() for v in r)
+        self.init_dof_pos_range, self.init_dof_vel_range = rng(self.init_dof_pos_range), rng(self.init_dof_vel_range)
+        self.motor_body = np.asarray(self.motor_body, np.int64)
+        self.motor_R, self.motor_p = np.asarray(self.motor_R, np.float64), np.asarray(self.motor_p, np.float64)
+        self.motor_torque = np.asarray(self.motor_torque, np.float64)
+        # a movable subtree without inertia about its axis and without a drive would make the joint's pivot D_i zero
+        d_tot = self.damping + b.urdf_damping[1:]
+        R0, P0 = [np.eye(3)], [np.zeros(3)]
+        for i in range(1, b.num_bodies):
+            l = b.parent[i]
+            R0.append(R0[l] @ b.joint_R[i])
+            P0.append(P0[l] + R0[l] @ b.joint_p[i])
+        for i in range(1, b.num_bodies):
+            if self.stiffness[i - 1] > 0 or d_tot[i - 1] > 0:
+                continue
+            a = R0[i] @ b.axis[i]
+            J = 0.0
+            for k in range(i, b.num_bodies):
+                anc = k
+                while anc > i:
+                    anc = b.parent[anc]
+                if anc != i:
+                    continue
+                r = P0[k] + R0[k] @ b.com[k] - P0[i]
+                Ic = R0[k] @ b.inertia[k] @ R0[k].T + b.mass[k] * (float(r @ r) * np.eye(3) - np.outer(r, r))
+                J += float(a @ Ic @ a)
+            if not J > 1e-12:
+                raise ValueError(f"joint '{b.joint_names[i]}': its subtree has no inertia about the axis and the joint has no drive "
+                                 "(stiffness = damping = 0), so its acceleration is undefined")
+
+    @property
+    def num_dofs(self) -> int:
+        return self.bodies.num_dofs
+
+    def to_struct(self) -> "_lib.AgxArticulation":
+        b, a = self.bodies, _lib.AgxArticulation()
+        a.num_bodies, a.num_dofs = b.num_bodies, b.num_dofs
+        for i in range(b.num_bodies):
+            a.parent[i] = int(b.parent[i])
+            _set(a.joint_R[i], b.joint_R[i]); _set(a.joint_p[i], b.joint_p[i]); _set(a.axis[i], b.axis[i])
+            a.mass[i] = float(b.mass[i])
+            _set(a.com[i], b.com[i]); _set(a.inertia[i], b.inertia[i])
+            a.lower[i], a.upper[i], a.limited[i] = float(b.lower[i]), float(b.upper[i]), int(bool(b.limited[i]))
+            if i > 0:
+                a.stiffness[i] = float(self.stiffness[i - 1])
+                a.damping[i] = float(self.damping[i - 1] + b.urdf_damping[i])
+        for k in range(len(self.motor_body)):
+            a.motor_body[k] = int(self.motor_body[k])
+            _set(a.motor_R[k], self.motor_R[k]); _set(a.motor_p[k], self.motor_p[k])
+            a.motor_torque[k] = float(self.motor_torque[k])
+        return a
+
+
 def _set(arr, vals):
     vals = np.asarray(vals, dtype=np.float64).reshape(-1)
     for i, v in enumerate(vals):
@@ -197,15 +273,19 @@ class Hp1Engine:
 
     def __init__(self, spec: MultirotorSpec, num_envs: int, device="cuda:0", *, physics_steps=1,
                  episode_len_steps=500, seed=0, env_id_offset=0, device_rng_reset=True, strict_stale_obs=True,
-                 materialize_derived=True, per_env_params="auto", debug_wrench=False, host_io=False):
+                 materialize_derived=True, per_env_params="auto", debug_wrench=False, host_io=False, articulation=None):
         """host_io: obs / reward / terminations / truncations live in pinned, device-mapped HOST
         memory (agx_host_alloc) and the fused task step stores them there directly over PCIe;
         `actions` may then be a pinned host tensor (e.g. `self.host_actions`) that the kernel
-        reads in place.  The caller synchronises the stream before reading the results."""
+        reads in place.  The caller synchronises the stream before reading the results.
+        articulation: an ArticulationSpec -- the robot has joints; physics_step runs agx_hp1_articulated_step and the engine owns
+        dof_state [N,D,2] and the drive targets dof_position_setpoint / dof_velocity_setpoint [N,D] (zero until the caller writes
+        them).  There is no fused task step for such a robot."""
         self.lib = _lib.load()
         self.device = torch.device(device)
         if self.device.type != "cuda":
             raise _lib.AgxError("Hp1Engine needs a CUDA device: there is no CPU path")
+        self._init_articulation(articulation, num_envs, debug_wrench, host_io)
         self.spec, self.N, self.M = spec, int(num_envs), spec.num_motors
         self.cfg = build_config(spec, self.N, physics_steps=physics_steps, episode_len_steps=episode_len_steps,
                                 seed=seed, env_id_offset=env_id_offset, device_rng_reset=device_rng_reset,
@@ -270,6 +350,25 @@ class Hp1Engine:
         self._task_step_gathered = self.lib.agx_hp1_position_task_step_gathered
 
     # ---- plumbing ---------------------------------------------------------------------------
+    def _init_articulation(self, articulation, num_envs, debug_wrench, host_io):
+        self.articulation, self.art = articulation, None
+        self.dof_state = self.dof_position_setpoint = self.dof_velocity_setpoint = None
+        if articulation is None:
+            return
+        if debug_wrench:
+            raise ValueError("an articulated robot has no single body wrench to report (debug_wrench)")
+        if host_io:
+            raise NotImplementedError("host_io is a feature of the fused task step, which articulated robots do not have")
+        N, D, dev = int(num_envs), articulation.num_dofs, self.device
+        self.dof_state = torch.zeros(N, D, 2, dtype=torch.float32, device=dev)
+        self.dof_position_setpoint = torch.zeros(N, D, dtype=torch.float32, device=dev)
+        self.dof_velocity_setpoint = torch.zeros(N, D, dtype=torch.float32, device=dev)
+        self.art = articulation.to_struct()
+        self.art.dof_state = self.dof_state.data_ptr()
+        self.art.dof_position_setpoint = self.dof_position_setpoint.data_ptr()
+        self.art.dof_velocity_setpoint = self.dof_velocity_setpoint.data_ptr()
+        self._art_ref = C.byref(self.art)
+
     def _host_tensor(self, shape, dtype):
         nbytes = max(1, int(np.prod(shape))) * torch.empty((), dtype=dtype).element_size()
         p = C.c_void_p()
@@ -400,11 +499,17 @@ class Hp1Engine:
         self._buf.dist_offset = dist_offset
         if physics_steps is not None:
             self.cfg.physics_steps = int(physics_steps)
+        if self.art is not None:
+            _lib.check(self.lib.agx_hp1_articulated_step(self._cfg_ref, self._buf_ref, self._art_ref, self._stream()),
+                       "agx_hp1_articulated_step")
+            return
         _lib.check(self.lib.agx_hp1_physics_step(self._cfg_ref, self._buf_ref, self._stream()), "agx_hp1_physics_step")
 
     def position_task_step(self, actions, disturbance=None, physics_steps=None, mid_event=None):
         """mid_event: optional torch.cuda.Event(enable_timing=True), already recorded once (so its
         handle exists); the library records it between the main kernel and the refresh pass."""
+        if self.art is not None:
+            raise ValueError("an articulated robot has no fused task step: step it with physics_step (PositionSetpointTask does)")
         self._check_actions(actions)
         self._buf.disturbance = None if disturbance is None else disturbance.data_ptr()
         self._buf.dist_counter = None

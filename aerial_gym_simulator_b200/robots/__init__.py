@@ -7,7 +7,7 @@ import numpy as np
 from .. import control  # noqa: F401  (registers controllers)
 from .. import urdf
 from ..config import robot_config as rc
-from ..hp1 import MultirotorSpec
+from ..hp1 import ArticulationSpec, MultirotorSpec
 from ..registry._core import controller_registry, robot_registry
 
 
@@ -102,6 +102,39 @@ class BaseROV(BaseMultirotor):
     keeps_motor_state_on_reset = True
 
 
+class ArticulatedMultirotor(BaseMultirotor):
+    """A multirotor whose URDF tree has revolute / continuous joints (DESIGN.md "Articulated robots").  The controller, allocation and
+    motor model are BaseMultirotor's, with the zero-configuration mass and inertia; the motors push on the bodies their links were
+    merged into, and the joints are driven towards the engine's dof_position_setpoint / dof_velocity_setpoint by the drive of the
+    config's joint_config (stiffness, damping per DOF; a scalar applies to every DOF)."""
+    articulated = True
+
+    def __init__(self, robot_config, controller_name, env_config, device):
+        super().__init__(robot_config, controller_name, env_config, device)
+        if self.force_application_level != "motor_link":
+            raise ValueError("an articulated robot needs force_application_level = 'motor_link': its motors push on the links "
+                             "they belong to ('root_link' would apply them to the base)")
+        self.bodies = self.urdf_model.articulation()  # raises for unsupported joints, zero axes and too many bodies
+
+    def make_articulation(self) -> ArticulationSpec:
+        ca, jc, b = self.cfg.control_allocator_config, self.cfg.joint_config, self.bodies
+        order = self.urdf_model.body_order()
+        M = ca.num_motors
+        mb, mR, mp = np.zeros(M, np.int64), np.zeros((M, 3, 3)), np.zeros((M, 3))
+        for i, idx in enumerate(ca.application_mask):
+            if idx >= len(order):
+                raise ValueError(f"application_mask entry {idx} exceeds the {len(order)} bodies of the URDF")
+            link = order[idx]
+            mb[i] = b.link_body[link]
+            mR[i], mp[i] = b.link_in_body[link]
+        cq = float(ca.motor_model_config.thrust_to_torque_ratio)
+        return ArticulationSpec(
+            bodies=b, stiffness=jc.stiffness, damping=jc.damping, motor_body=mb, motor_R=mR, motor_p=mp,
+            motor_torque=-cq * np.asarray(ca.motor_directions, np.float64),
+            init_dof_pos_range=(jc.min_init_dof_position, jc.max_init_dof_position),
+            init_dof_vel_range=(jc.min_init_dof_velocity, jc.max_init_dof_velocity))
+
+
 for _name, _cfg in (
     ("base_quadrotor", rc.BaseQuadCfg), ("base_octarotor", rc.BaseOctarotorCfg),
     ("base_quad_root_link_control", rc.BaseQuadRootLinkControlCfg), ("lmf1", rc.LMF1Cfg), ("lmf2", rc.LMF2Cfg),
@@ -113,6 +146,7 @@ for _name, _cfg in (
 ):
     robot_registry.register(_name, BaseMultirotor, _cfg)
 robot_registry.register("base_rov", BaseROV, rc.BaseROVCfg)
+robot_registry.register("morphy_compliant", ArticulatedMultirotor, rc.MorphyCompliantCfg)
 
 # the reference's package also exports its robot config classes (robots/__init__.py: `from ...base_quad_config import *`, ...)
 globals().update({_k: _v for _k, _v in vars(rc).items() if _k.endswith("Cfg")})

@@ -48,6 +48,8 @@ class PositionSetpointTask(BaseTask):
         # here, once, so that no step consumes random.gauss and then fails)
         e = env.cfg.env
         self._unfused = bool(env.spec.enable_disturbance and (e.num_physics_steps_per_env_step_mean != 1 or e.num_physics_steps_per_env_step_std != 0))
+        # an articulated robot has no fused step: its physics is agx_hp1_articulated_step, the rest of the step the same sequence
+        self._unfused = self._unfused or env.articulated
         self.actions = torch.zeros((self.num_envs, self.task_config.action_space_dim), device=self.device)
         self.prev_actions = torch.zeros_like(self.actions)
         self.counter = 0

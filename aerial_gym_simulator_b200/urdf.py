@@ -60,6 +60,44 @@ class Joint:
     R: np.ndarray
     p: np.ndarray
     kind: str = "fixed"
+    axis: np.ndarray = field(default_factory=lambda: np.array([1.0, 0.0, 0.0]))  # <axis xyz>, joint frame, as written
+    lower: float = 0.0  # <limit lower upper>
+    upper: float = 0.0
+    damping: float = 0.0  # <dynamics damping>
+
+
+MOVABLE_JOINTS = ("revolute", "continuous")
+
+
+@dataclass
+class ArticulatedBodies:
+    """The links of a URDF merged across its fixed joints into rigid bodies (UrdfModel.articulation).  Body 0 is the root link's; body
+    i >= 1 hangs on one movable joint (DOF i - 1) and its frame is the frame of that joint's child link.  Bodies are numbered in
+    body_order()'s depth-first order, so every parent precedes its children."""
+    links: List[str]             # the link each body's frame is, [B]
+    parent: np.ndarray           # [B] int, parent body (-1 for body 0)
+    joint_names: List[str]       # [B] ("" for body 0)
+    joint_kinds: List[str]
+    joint_R: np.ndarray          # [B,3,3] parent body frame -> body frame at q = 0
+    joint_p: np.ndarray          # [B,3]
+    axis: np.ndarray             # [B,3] unit, body frame
+    lower: np.ndarray            # [B]
+    upper: np.ndarray
+    limited: np.ndarray          # [B] bool: revolute with lower < upper
+    urdf_damping: np.ndarray     # [B] <dynamics damping>
+    mass: np.ndarray             # [B]
+    com: np.ndarray              # [B,3] body frame
+    inertia: np.ndarray          # [B,3,3] about the COM, body axes
+    link_body: Dict[str, int]    # body each link was merged into
+    link_in_body: Dict[str, Tuple[np.ndarray, np.ndarray]]  # (R, p) of each link in its body's frame
+
+    @property
+    def num_bodies(self) -> int:
+        return len(self.links)
+
+    @property
+    def num_dofs(self) -> int:
+        return len(self.links) - 1
 
 
 @dataclass
@@ -120,6 +158,61 @@ class UrdfModel:
             J += Rl @ l.inertia @ Rl.T + l.mass * (float(d @ d) * np.eye(3) - np.outer(d, d))
         return m_tot, com, J
 
+    def articulation(self, max_bodies: int = 16) -> ArticulatedBodies:
+        """The merged body table of an articulated robot.  Each body's mass, COM and inertia are the parallel-axis accumulation of
+        composite_inertia() over the links merged into it.  Joints other than fixed / revolute / continuous, a zero <axis> and more
+        than `max_bodies` bodies raise ValueError."""
+        by_child = {j.child: j for j in self.joints}
+        names, parent, jn, jk, jR, jp, ax, lo, hi, lim, dmp = [], [], [], [], [], [], [], [], [], [], []
+        link_body, link_in_body = {}, {}
+        for name in self.body_order():
+            j = by_child.get(name)
+            if j is None or j.kind == "fixed":
+                if j is None:
+                    b, T = 0, (np.eye(3), np.zeros(3))
+                    names.append(name); parent.append(-1); jn.append(""); jk.append("")
+                    jR.append(np.eye(3)); jp.append(np.zeros(3)); ax.append(np.zeros(3))
+                    lo.append(0.0); hi.append(0.0); lim.append(False); dmp.append(0.0)
+                else:
+                    b = link_body[j.parent]
+                    Rp, pp = link_in_body[j.parent]
+                    T = (Rp @ j.R, pp + Rp @ j.p)
+                link_body[name], link_in_body[name] = b, T
+                continue
+            if j.kind not in MOVABLE_JOINTS:
+                raise ValueError(f"joint '{j.name}' is {j.kind}: articulated robots support revolute and continuous joints only")
+            a = np.asarray(j.axis, dtype=np.float64)
+            n = float(np.linalg.norm(a))
+            if not n > 0:
+                raise ValueError(f"joint '{j.name}' has a zero <axis>")
+            Rp, pp = link_in_body[j.parent]
+            link_body[name], link_in_body[name] = len(names), (np.eye(3), np.zeros(3))
+            names.append(name); parent.append(link_body[j.parent]); jn.append(j.name); jk.append(j.kind)
+            jR.append(Rp @ j.R); jp.append(pp + Rp @ j.p); ax.append(a / n)
+            limited = j.kind == "revolute" and j.lower < j.upper
+            lo.append(float(j.lower)); hi.append(float(j.upper)); lim.append(limited); dmp.append(float(j.damping))
+        B = len(names)
+        if B > max_bodies:
+            raise ValueError(f"{B} bodies after merging the fixed joints: at most {max_bodies} are supported ({max_bodies - 1} DOFs)")
+        mass, com, inertia = np.zeros(B), np.zeros((B, 3)), np.zeros((B, 3, 3))
+        csum = np.zeros((B, 3))
+        for name, b in link_body.items():
+            l = self.links[name]
+            R, p = link_in_body[name]
+            mass[b] += l.mass
+            csum[b] += l.mass * (p + R @ l.com)
+        for b in range(B):
+            com[b] = csum[b] / mass[b] if mass[b] > 0 else np.zeros(3)
+        for name, b in link_body.items():
+            l = self.links[name]
+            R, p = link_in_body[name]
+            Rl = R @ l.com_R
+            d = (p + R @ l.com) - com[b]
+            inertia[b] += Rl @ l.inertia @ Rl.T + l.mass * (float(d @ d) * np.eye(3) - np.outer(d, d))
+        return ArticulatedBodies(names, np.asarray(parent, np.int64), jn, jk, np.asarray(jR), np.asarray(jp), np.asarray(ax),
+                                 np.asarray(lo), np.asarray(hi), np.asarray(lim, bool), np.asarray(dmp), mass, com, inertia,
+                                 link_body, link_in_body)
+
 
 def _parse_geometry(el, base_dir) -> Optional[Visual]:
     geom = el.find("geometry")
@@ -178,6 +271,13 @@ def parse_urdf(path: str) -> UrdfModel:
         R = rpy_to_matrix(_vec(org.get("rpy") if org is not None else None))
         p = _vec(org.get("xyz") if org is not None else None)
         j = Joint(je.get("name"), je.find("parent").get("link"), je.find("child").get("link"), R, p, je.get("type", "fixed"))
+        ae, le, de = je.find("axis"), je.find("limit"), je.find("dynamics")
+        if ae is not None and ae.get("xyz") is not None:
+            j.axis = _vec(ae.get("xyz"))
+        if le is not None:
+            j.lower, j.upper = float(le.get("lower", 0.0)), float(le.get("upper", 0.0))
+        if de is not None:
+            j.damping = float(de.get("damping", 0.0))
         joints.append(j)
         children.add(j.child)
     roots = [n for n in links if n not in children]

@@ -173,7 +173,7 @@ const char* agx_last_error(void);
 /* sizeof() of the ABI structs as compiled into the library (binding self-check):
  * which = 0 AgxHp1Config, 1 AgxHp1Buffers, 2 AgxHp1ResetDraws, 3 AgxHp2Scene, 4 AgxHp2Sensor,
  * 5 AgxNavRewardParams, 6 AgxImuConfig, 7 AgxLidarNavRewardParams, 8 AgxHp2Noise, 9 AgxE2ERewardParams, 10 AgxObsGatherPush,
- * 11 AgxContactParams, 12 AgxContactMotion, 13 AgxObstacleMass, 14 AgxObstacleHull */
+ * 11 AgxContactParams, 12 AgxContactMotion, 13 AgxObstacleMass, 14 AgxObstacleHull, 15 AgxArticulation */
 uint64_t agx_sizeof(int which);
 
 /* Host buffers the kernels can address directly (pinned, portable, mapped: cudaHostAlloc).
@@ -225,6 +225,44 @@ int agx_set_spin_timeout_ms(uint64_t ms);
 int agx_counter_add(uint32_t* counter, uint32_t n, void* stream);
 /* Synchronises `stream` and returns AGX_E_TIMEOUT if a wait of the chained step expired since any_reset was zeroed. */
 int agx_hp1_check(const AgxHp1Buffers* buf, void* stream);
+
+/* ---- articulated multirotors (DESIGN.md "Articulated robots") ------------------------------------------------------------
+ * A URDF tree merged across its fixed joints into rigid bodies, numbered parent before child; body 0 is the floating base (the
+ * root link's body, whose row in root_state keeps its meaning), body i >= 1 hangs on one revolute / continuous joint, DOF i - 1.
+ * Body frame = the frame of the link the body's joint points at (the root link for body 0).  Shared by all envs except the three
+ * [N,...] device arrays. */
+#define AGX_ART_MAX_BODIES 16
+typedef struct AgxArticulation {
+    int32_t num_bodies;                      /* B in [1, AGX_ART_MAX_BODIES] */
+    int32_t num_dofs;                        /* D = B - 1 */
+    int32_t parent[AGX_ART_MAX_BODIES];      /* parent body (< i); parent[0] = -1 */
+    float joint_R[AGX_ART_MAX_BODIES][9];    /* parent body frame -> body frame at q = 0, row-major (body 0: identity) */
+    float joint_p[AGX_ART_MAX_BODIES][3];    /* body origin in the parent body frame */
+    float axis[AGX_ART_MAX_BODIES][3];       /* joint axis, unit, body frame */
+    float mass[AGX_ART_MAX_BODIES];
+    float com[AGX_ART_MAX_BODIES][3];        /* body frame */
+    float inertia[AGX_ART_MAX_BODIES][9];    /* about the COM, body-frame axes, row-major */
+    float lower[AGX_ART_MAX_BODIES];         /* joint limits; projected only where limited[i] != 0 */
+    float upper[AGX_ART_MAX_BODIES];
+    int32_t limited[AGX_ART_MAX_BODIES];
+    float stiffness[AGX_ART_MAX_BODIES];     /* drive k [N m / rad] */
+    float damping[AGX_ART_MAX_BODIES];       /* drive d + URDF <dynamics damping> [N m s / rad] */
+    int32_t motor_body[AGX_MAX_MOTORS];      /* body each motor's application_mask link was merged into */
+    float motor_R[AGX_MAX_MOTORS][9];        /* motor link frame in that body's frame */
+    float motor_p[AGX_MAX_MOTORS][3];
+    float motor_torque[AGX_MAX_MOTORS];      /* reaction torque per unit thrust about the motor z axis: -thrust_to_torque_ratio * dir */
+    float* dof_state;                        /* [N,D,2] (position, velocity), read and written */
+    const float* dof_position_setpoint;      /* [N,D] drive targets q*, q-dot* */
+    const float* dof_velocity_setpoint;
+} AgxArticulation;
+
+/* agx_hp1_physics_step for an articulated robot: `physics_steps` x (update_states of the base -> controller -> allocation -> motor
+ * model, as agx_hp1_physics_step; then forward kinematics, every motor's thrust and reaction torque on the body its link belongs
+ * to, drag and disturbance on the base, gravity on every body, the floating-base articulated-body algorithm with the implicit joint
+ * drive, the base integrated by the HP1 integrator spec, q-dot += dt q-ddot, q += dt q-dot, limit projection).  Same buffers,
+ * derived states and in-kernel disturbance draw as agx_hp1_physics_step; buf->body_wrench must be NULL.  Capturable: no
+ * allocation, no synchronisation. */
+int agx_hp1_articulated_step(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, const AgxArticulation* art, void* stream);
 
 /* Masked re-initialisation, EnvManager.reset_idx for a robot-only scene
  * (env_manager/env_manager.py:273-301 -> IGE_env_manager.py:513-519, base_multirotor.py:177-205,
