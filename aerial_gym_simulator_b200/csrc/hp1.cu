@@ -32,22 +32,14 @@ constexpr int kThreads = kWarpsPerBlock * 32;
 constexpr int kTileFloats = 32 * 13;
 
 
-__device__ __forceinline__ uint32_t ld_acquire_gpu_u32(const uint32_t* p) {
-    uint32_t v;
-    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void fence_acq_rel_gpu() { asm volatile("fence.acq_rel.gpu;" ::: "memory"); }
+// The chain handshake polls with RELAXED loads and acquires once, with a fence, after the wait: on sm_90a every acquire (an
+// ld.acquire, or the acquire half of fence.acq_rel) is followed by CCTL.IVALL, which invalidates the SM's whole L1 -- and with it the
+// stack lines of every warp on the SM.  fence.acquire costs that invalidation once per wait instead of once per poll, and
+// fence.release is a MEMBAR without one.
+__device__ __forceinline__ void fence_acquire_gpu() { asm volatile("fence.acquire.gpu;" ::: "memory"); }
+__device__ __forceinline__ void fence_release_gpu() { asm volatile("fence.release.gpu;" ::: "memory"); }
 __device__ __forceinline__ void st_relaxed_gpu_u32(uint32_t* p, uint32_t v) {
     asm volatile("st.relaxed.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ void st_release_gpu_u32(uint32_t* p, uint32_t v) {
-    asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ unsigned long long ld_acquire_gpu_u64(const unsigned long long* p) {
-    unsigned long long v;
-    asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-    return v;
 }
 __device__ __forceinline__ uint32_t ld_relaxed_gpu_u32(const uint32_t* p) {
     uint32_t v;
@@ -94,9 +86,9 @@ __device__ __forceinline__ bool spin_until(Pred ok, int32_t* any_reset, int code
 }
 
 // ---- tile IO ---------------------------------------------------------------------------
-// rows [env0, env0+n_valid) of a dense [N,13] array -> this lane's row in r[13]
-__device__ __forceinline__ void load_rows13(const float* __restrict__ base, int env0, int n_valid,
-                                            float* tile, int lane, float r[13], bool vec_ok) {
+// rows [env0, env0+n_valid) of a dense [N,13] array -> the tile (row `lane` for lane `lane`)
+__device__ __forceinline__ void fill_rows13(const float* __restrict__ base, int env0, int n_valid, float* tile, int lane,
+                                            bool vec_ok) {
     const float* src = base + (size_t)env0 * 13;
     if (n_valid == 32 && vec_ok) {
         const float4* s4 = reinterpret_cast<const float4*>(src);
@@ -111,18 +103,20 @@ __device__ __forceinline__ void load_rows13(const float* __restrict__ base, int 
         for (int i = lane; i < n; i += 32) tile[i] = __ldcg(src + i);
     }
     __syncwarp();
+}
+// rows [env0, env0+n_valid) of a dense [N,13] array -> this lane's row in r[13]
+__device__ __forceinline__ void load_rows13(const float* __restrict__ base, int env0, int n_valid,
+                                            float* tile, int lane, float r[13], bool vec_ok) {
+    fill_rows13(base, env0, n_valid, tile, lane, vec_ok);
     if (lane < n_valid) {
 #pragma unroll
         for (int j = 0; j < 13; ++j) r[j] = tile[lane * 13 + j];
     }
     __syncwarp();
 }
-__device__ __forceinline__ void store_rows13(float* __restrict__ base, int env0, int n_valid, float* tile,
-                                             int lane, const float r[13], bool vec_ok) {
-    if (lane < n_valid) {
-#pragma unroll
-        for (int j = 0; j < 13; ++j) tile[lane * 13 + j] = r[j];
-    }
+// the tile (row `lane` written by lane `lane`) -> rows [env0, env0+n_valid) of a dense [N,13] array
+__device__ __forceinline__ void flush_rows13(float* __restrict__ base, int env0, int n_valid, const float* tile, int lane,
+                                             bool vec_ok) {
     __syncwarp();
     float* dst = base + (size_t)env0 * 13;
     if (n_valid == 32 && vec_ok) {
@@ -138,6 +132,14 @@ __device__ __forceinline__ void store_rows13(float* __restrict__ base, int env0,
         for (int i = lane; i < n; i += 32) dst[i] = tile[i];
     }
     __syncwarp();
+}
+__device__ __forceinline__ void store_rows13(float* __restrict__ base, int env0, int n_valid, float* tile,
+                                             int lane, const float r[13], bool vec_ok) {
+    if (lane < n_valid) {
+#pragma unroll
+        for (int j = 0; j < 13; ++j) tile[lane * 13 + j] = r[j];
+    }
+    flush_rows13(base, env0, n_valid, tile, lane, vec_ok);
 }
 template <int M>
 __device__ __forceinline__ void load_m(const float* __restrict__ p, int env, float out[M]) {
@@ -256,8 +258,8 @@ AGX_HP1_RESET_FN void reset_one_env(const AgxHp1Config& cfg, const AgxHp1Buffers
 // chained per TILE, not per grid: launched with programmatic stream serialization, a step's CTAs are
 // scheduled while the previous step's slower warps are still running, each warp takes its step number T
 // from a per-tile claim counter (atomicAdd, before the CTA triggers its dependents, so claims are in launch
-// order), spins until its tile's done-counter says step T-1 has been published (st.release after the last
-// store / ld.acquire before the first L2-only load), and runs.  The launch's tail (slow SMs, the ~6 % of
+// order), spins until its tile's done-counter says step T-1 has been published (fence.release after the last
+// store / relaxed polls, then one fence.acquire before the first L2-only load), and runs.  The launch's tail (slow SMs, the ~6 % of
 // warps with a resetting env) no longer gates the next step.  A warp also waits until step T-2 is complete
 // everywhere, so at most two consecutive steps are in flight and four parity slots suffice:
 //   any_reset[4 + (T & 3)]        u32 flag of step T: raised = holds T + 1 (monotonic, never cleared)
@@ -301,7 +303,6 @@ hp1_step_kernel(const __grid_constant__ AgxHp1Config cfg, const __grid_constant_
     AGX_TL(0);
     uint32_t* reset_flag = reinterpret_cast<uint32_t*>(buf.any_reset);
     unsigned long long* arrive_ctr = nullptr;
-    unsigned long long* publish_ctr = nullptr;
     unsigned long long arrive_target = 0;  // arrivals once every warp of this step has counted itself in
     uint32_t step_T = 0;
     if constexpr (COOP) {
@@ -318,19 +319,19 @@ hp1_step_kernel(const __grid_constant__ AgxHp1Config cfg, const __grid_constant_
             if (lane == 0) {
                 const uint32_t* done = buf.tile_sync + n_tiles + my_tile;
                 // this tile's previous step has published its state
-                spin_until([&] { return ld_acquire_gpu_u32(done) == step_T; }, buf.any_reset, 1 | (int)(step_T << 4));
+                spin_until([&] { return ld_relaxed_gpu_u32(done) == step_T; }, buf.any_reset, 1 | (int)(step_T << 4));
                 if (step_T >= 2u) {  // step T-2 complete everywhere: bounds the skew to two steps in flight
                     const uint32_t P = step_T - 2u;
                     const unsigned long long* a2 = reinterpret_cast<const unsigned long long*>(buf.any_reset + 8) + (P & 3u);
                     const unsigned long long want2 = (unsigned long long)(P / 4u + 1u) * (unsigned long long)n_tiles;
-                    spin_until([&] { return ld_acquire_gpu_u64(a2) >= want2; }, buf.any_reset, 2 | (int)(step_T << 4));
+                    spin_until([&] { return ld_relaxed_gpu_u64(a2) >= want2; }, buf.any_reset, 2 | (int)(step_T << 4));
                 }
+                fence_acquire_gpu();  // one acquire for both waits, before the warp's first load of the tile
             }
             __syncwarp();
         }
         reset_flag = reinterpret_cast<uint32_t*>(buf.any_reset) + 4 + (step_T & 3u);
         arrive_ctr = reinterpret_cast<unsigned long long*>(buf.any_reset + 8) + (step_T & 3u);
-        publish_ctr = buf.publish_ctr ? buf.publish_ctr + (step_T & 3u) : nullptr;
         arrive_target = (unsigned long long)(step_T / 4u + 1u) * (unsigned long long)n_tiles;
     }
     const uint32_t flag_tag = step_T + 1u;
@@ -350,7 +351,6 @@ hp1_step_kernel(const __grid_constant__ AgxHp1Config cfg, const __grid_constant_
         // latencies overlap (the kernel is latency bound at 65,536 envs)
         EnvParams<M> p;
         float act[AGX_MAX_MOTORS];
-        float Fx = 0, Fy = 0, Fz = 0, Tx = 0, Ty = 0, Tz = 0;
         int steps_in = 0;
         tgt = V3{0.f, 0.f, 0.f};
         if (valid) {
@@ -372,8 +372,7 @@ hp1_step_kernel(const __grid_constant__ AgxHp1Config cfg, const __grid_constant_
 #pragma unroll
             for (int i = 0; i < AGX_MAX_MOTORS; ++i) act[i] = fminf(fmaxf(act[i], -10.0f), 10.0f);
         }
-        float r[13];
-        load_rows13(buf.root_state, env0, n_valid, tile, lane, r, vec_ok);
+        fill_rows13(buf.root_state, env0, n_valid, tile, lane, vec_ok);
         if constexpr (COOP) {  // truncations are known before the physics: publish them now
             const bool trunc_early = valid && (steps_in + 1 > cfg.episode_len_steps);
             if (__ballot_sync(0xffffffffu, trunc_early)) {
@@ -381,13 +380,15 @@ hp1_step_kernel(const __grid_constant__ AgxHp1Config cfg, const __grid_constant_
                 if (lane == 0) atomicMax(reset_flag, flag_tag);
             }
         }
+        // the state is read from the tile only now: its 13 floats are not live across the loads' wait and the ballot above
+        if (valid) s = unpack(tile + lane * 13);
+        __syncwarp();
         if (valid) {
-            s = unpack(r);
-
             // every iteration runs the same instruction sequence, so n fused sub-steps are
             // bit-identical to n single-step launches
 #pragma unroll 1
             for (int step = 0; step < cfg.physics_steps; ++step) {
+                float Fx, Fy, Fz, Tx, Ty, Tz;
                 // AGX_SHADOW_BEGIN(physics_substep)  -- tests/_shadow.py compiles the text between these markers for the host
                 d = update_states(s);
                 float ref[M];
@@ -441,8 +442,19 @@ AGX_HP1_MOTOR_UNROLL
                 Fx = F.x; Fy = F.y; Fz = F.z; Tx = T.x; Ty = T.y; Tz = T.z;
                 integrate<SP>(cfg, s, F, T);
                 // AGX_SHADOW_END(physics_substep)
+                // the last sub-step's wrench is stored here: held for after the loop, its six floats were live through every sub-step
+                if (buf.body_wrench && step + 1 == cfg.physics_steps) {
+                    float* bw = buf.body_wrench + (size_t)env * 6;
+                    bw[0] = Fx; bw[1] = Fy; bw[2] = Fz; bw[3] = Tx; bw[4] = Ty; bw[5] = Tz;
+                }
             }
-            if (cfg.physics_steps == 0) d = update_states(s);
+            if (cfg.physics_steps == 0) {
+                d = update_states(s);
+                if (buf.body_wrench) {
+                    float* bw = buf.body_wrench + (size_t)env * 6;
+                    bw[0] = 0.f; bw[1] = 0.f; bw[2] = 0.f; bw[3] = 0.f; bw[4] = 0.f; bw[5] = 0.f;
+                }
+            }
         }
 
         AGX_TL(1);
@@ -523,12 +535,16 @@ AGX_HP1_MOTOR_UNROLL
                     volatile uint32_t* fl = reset_flag;
                     const unsigned long long* cnt = arrive_ctr;
                     // until the flag rises, or every warp of this step has arrived (then the flag is final)
-                    spin_until([&] { return *fl == flag_tag || ld_acquire_gpu_u64(cnt) >= arrive_target; }, buf.any_reset, 3 | (int)(step_T << 4));
+                    spin_until([&] { return *fl == flag_tag || ld_relaxed_gpu_u64(cnt) >= arrive_target; }, buf.any_reset, 3 | (int)(step_T << 4));
+                    fence_acquire_gpu();  // a complete count orders every warp's raised flag before the re-read below
                     any = __any_sync(0xffffffffu, *fl == flag_tag);  // the flag is monotonic: one lane seeing it raised means it is
                 }
                 // ---- derived states for the observation: one common pass for resetting envs (new state)
                 // and, if anybody reset, for everybody else (post-physics state) ------------------------
                 const bool derived = buf.euler || buf.vehicle_orientation || buf.vehicle_linvel || buf.body_linvel || buf.body_angvel;
+                // the root-state row, then the observation row, is written straight into the tile: no 13-float copy of either is
+                // held in registers next to s, d and p (the register budget is full here: they were the epilogue's spills)
+                float* row = tile + lane * 13;
                 if (valid) {
                     if (fresh || any) {
                         if (derived) {
@@ -538,38 +554,33 @@ AGX_HP1_MOTOR_UNROLL
                             d.wb = quat_rotate_inverse(s.q, s.w);
                         }
                     }
-                    make_obs(s, d, tgt, o);
                     store_m<M>(buf.motor_thrust, env, p.thrust);
                     if (derived) store_derived(buf, env, d);
-                    if (buf.body_wrench) {
-                        float* bw = buf.body_wrench + (size_t)env * 6;
-                        bw[0] = Fx; bw[1] = Fy; bw[2] = Fz; bw[3] = Tx; bw[4] = Ty; bw[5] = Tz;
-                    }
-                    pack(s, r);
+                    pack(s, row);
                 }
-                store_rows13(buf.root_state, env0, n_valid, tile, lane, r, vec_ok);
-                store_rows13(buf.obs, env0, n_valid, tile, lane, o, vec_ok);
-                __syncwarp();
+                flush_rows13(buf.root_state, env0, n_valid, tile, lane, vec_ok);
+                if (valid) make_obs(s, d, tgt, row);
+                flush_rows13(buf.obs, env0, n_valid, tile, lane, vec_ok);
                 if (lane == 0) {
                     // ONE release fence (MEMBAR.ALL.GPU), then relaxed operations: the tile's stores (and a raised flag) are visible before
                     // the arrival, the publish count and the done-counter (fence-based release; the consumers acquire).  Round 1 had
                     // __threadfence() (MEMBAR.SC + L1 invalidate) followed by st.release (a second MEMBAR): ncu r2 showed `membar` as the
-                    // second largest stall of the kernel.
-                    fence_acq_rel_gpu();
+                    // second largest stall of the kernel.  Nothing after it reads what another warp wrote, so it needs no acquire half
+                    // (fence.acq_rel would add an L1 invalidation).
+                    fence_release_gpu();
                     if (!counted) atomicAdd(arrive_ctr, 1ull);
-                    if (publish_ctr) atomicAdd(publish_ctr, 1ull);  // only with a consumer outside the kernel (observation gather)
+                    // only with a consumer outside the kernel (observation gather); the address is formed here, not held in a register
+                    // (or a spill slot) for the whole step
+                    if (buf.publish_ctr) atomicAdd(buf.publish_ctr + (step_T & 3u), 1ull);
                     st_relaxed_gpu_u32(buf.tile_sync + n_tiles + t, flag_tag);  // this tile may start step T + 1
                 }
             }
         }
         if constexpr (!(TASK && COOP)) {
+            float r[13];
             if (valid) {
                 store_m<M>(buf.motor_thrust, env, p.thrust);
                 store_derived(buf, env, d);
-                if (buf.body_wrench) {
-                    float* bw = buf.body_wrench + (size_t)env * 6;
-                    bw[0] = Fx; bw[1] = Fy; bw[2] = Fz; bw[3] = Tx; bw[4] = Ty; bw[5] = Tz;
-                }
                 pack(s, r);
             }
             store_rows13(buf.root_state, env0, n_valid, tile, lane, r, vec_ok);
