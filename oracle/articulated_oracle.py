@@ -8,8 +8,15 @@ follows the articulated-body recursion of articulated_core.cuh.
 Conventions shared with the product (they define what is compared, not how it is computed): spatial vectors in world axes about the
 base origin O, angular part first; generalised velocity = (base twist at O, q-dot); a0 = the base's spatial acceleration at O.
 `table` is a dict of numpy arrays with the fields of AgxArticulation (num_bodies, parent, joint_R [B,3,3], joint_p, axis, mass, com,
-inertia [B,3,3], stiffness, damping, motor_body, motor_R [M,3,3], motor_p, motor_torque)."""
+inertia [B,3,3], stiffness, damping, motor_body, motor_R [M,3,3], motor_p, motor_torque; integrate() also reads lower, upper,
+limited [B]).
+
+substep() is one whole sub-step of the articulated step (articulated_core.cuh's art_env_step): the controller, allocation, motor
+model, drag and derived states of oracle/hp1_oracle.py run in float64, then dynamics() and integrate() below."""
 import numpy as np
+import torch
+
+from . import hp1_oracle as HO
 
 
 def _skew(v):
@@ -112,6 +119,80 @@ def dynamics(table, root, q, qd, qs, qds, dt, grav, thrust, F_w, T_w):
     tau[6:] = k * (qs - q - dt * qd) + d * (qds - qd)
     x = np.linalg.solve(H, tau - C)
     return x[:6], x[6:]
+
+
+def _quat_mul(a, b):
+    """Hamilton product of xyzw quaternions"""
+    av, aw, bv, bw = a[:3], a[3], b[:3], b[3]
+    return np.concatenate([aw * bv + bw * av + np.cross(av, bv), [aw * bw - av @ bv]])
+
+
+def integrate(model, table, root, a0, q, qd, qdd):
+    """DESIGN.md section 3 on the base with the ABA's accelerations, then the joints of section 6 "Integration", one env.
+    model: hp1_oracle.Hp1Model (dt, damping, caps).  -> (root' [13], q' [D], qd' [D], q_free [D] = q' before the limit projection)"""
+    dt = model.dt
+    root = np.asarray(root, np.float64)
+    x, quat, v, w = root[0:3], root[3:7], root[7:10], root[10:13]
+    R = quat_to_matrix(quat)
+    a = a0[3:] + np.cross(w, v)  # the classical acceleration of the base origin
+    v1 = (v + dt * a) * max(0.0, 1.0 - dt * model.linear_damping)
+    vn = np.linalg.norm(v1)
+    if vn > model.max_linear_velocity:
+        v1 = v1 * (model.max_linear_velocity / vn)
+    W = R.T @ w
+    W1 = W + dt * (R.T @ a0[:3])
+    w1 = (R @ W1) * max(0.0, 1.0 - dt * model.angular_damping)
+    wn = np.linalg.norm(w1)
+    if wn > model.max_angular_velocity:
+        w1 = w1 * (model.max_angular_velocity / wn)
+        wn = np.linalg.norm(w1)
+    x1 = x + dt * v1
+    so = np.sin(0.5 * dt * wn) / wn if wn > 0 else 0.0
+    qn = _quat_mul(np.concatenate([w1 * so, [np.cos(0.5 * dt * wn)]]), quat)
+    qn = qn / np.linalg.norm(qn)
+    # joints: semi-implicit, then the projection onto [lower, upper] of a limited joint
+    v1j = qd + dt * qdd
+    q1 = q + dt * v1j
+    q_free = q1.copy()
+    B = int(table["num_bodies"])
+    for j in range(B - 1):
+        if table["limited"][j + 1]:
+            lo, hi = table["lower"][j + 1], table["upper"][j + 1]
+            if q1[j] <= lo:
+                q1[j], v1j[j] = lo, max(v1j[j], 0.0)
+            if q1[j] >= hi:
+                q1[j], v1j[j] = hi, min(v1j[j], 0.0)
+    return np.concatenate([x1, qn, v1, w1]), q1, v1j, q_free
+
+
+def substep(model, table, st, q, qd, qs, qds, actions, disturbance=None):
+    """One sub-step of the articulated step for N envs in float64.
+
+    model: hp1_oracle.Hp1Model of the engine's MultirotorSpec; st: hp1_oracle.Hp1State in float64 (root [N,13], thrust and the
+    motor constants / gains the kernel reads); q, qd, qs, qds [N,D]; actions [N,A]; disturbance: [N,6] body-frame wrench or None.
+    The drag and disturbance act at the base origin, rotated to world axes.
+    -> dict: root [N,13], q, qd, q_free [N,D], thrust [N,M], derived (update_states at the sub-step's start), a0 [N,6], qdd [N,D]"""
+    f64 = lambda a: torch.as_tensor(np.asarray(a), dtype=torch.float64)
+    root = st.root
+    N, D = root.shape[0], int(table["num_bodies"]) - 1
+    d = HO.update_states(root)
+    cmd = HO.controller_wrench(model, st, d, torch.clamp(f64(actions), -10.0, 10.0))
+    ref = cmd if model.controller == HO.CTRL_NONE else cmd @ model.pinv_allocation(torch.float64).T
+    thrust = HO.motor_update(model, st, ref)
+    df, dtq = HO.drag_wrench(model, d)
+    if disturbance is not None:
+        df, dtq = df + f64(disturbance)[:, 0:3], dtq + f64(disturbance)[:, 3:6]
+    F_w, T_w = HO.quat_rotate(root[:, 3:7], df).numpy(), HO.quat_rotate(root[:, 3:7], dtq).numpy()
+    q, qd, qs, qds = (np.asarray(a, np.float64).reshape(N, D) for a in (q, qd, qs, qds))
+    out = {k: np.zeros(s) for k, s in (("root", (N, 13)), ("q", (N, D)), ("qd", (N, D)), ("q_free", (N, D)), ("a0", (N, 6)),
+                                        ("qdd", (N, D)))}
+    r, th = root.numpy(), thrust.numpy()
+    for n in range(N):
+        a0, qdd = dynamics(table, r[n], q[n], qd[n], qs[n], qds[n], model.dt, model.gravity, th[n], F_w[n], T_w[n])
+        out["a0"][n], out["qdd"][n] = a0, qdd
+        out["root"][n], out["q"][n], out["qd"][n], out["q_free"][n] = integrate(model, table, r[n], a0, q[n], qd[n], qdd)
+    out["thrust"], out["derived"] = th, {k: v.numpy() for k, v in d.items()}
+    return out
 
 
 def momentum(table, root, q, qd):

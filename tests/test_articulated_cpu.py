@@ -12,8 +12,10 @@ import torch
 from aerial_gym_simulator_b200 import _lib, urdf
 from aerial_gym_simulator_b200.hp1 import ArticulationSpec, MultirotorSpec
 from oracle import articulated_oracle as AO
+from oracle import hp1_oracle as HO
 
 from . import _articulated_shadow
+from . import _hp1_common as H
 from ._cpu_stack import CpuHp1Engine
 from ._cpu_stack_articulated import CpuArticulatedHp1Engine, articulated_cpu_stack
 from ._hp1_common import spec_from_registry
@@ -34,7 +36,8 @@ def table_of(s):
     return {"num_bodies": B, "parent": np.ctypeslib.as_array(s.parent).copy(), "joint_R": f(s.joint_R, 3, 3), "joint_p": f(s.joint_p, 3),
             "axis": f(s.axis, 3), "mass": f(s.mass), "com": f(s.com, 3), "inertia": f(s.inertia, 3, 3), "stiffness": f(s.stiffness),
             "damping": f(s.damping), "motor_body": np.ctypeslib.as_array(s.motor_body).copy(), "motor_R": f(s.motor_R, 3, 3),
-            "motor_p": f(s.motor_p, 3), "motor_torque": f(s.motor_torque)}
+            "motor_p": f(s.motor_p, 3), "motor_torque": f(s.motor_torque), "lower": f(s.lower), "upper": f(s.upper),
+            "limited": np.ctypeslib.as_array(s.limited).copy()}
 
 
 def shadow_dynamics(s, root, q, qd, qs, qds, dt, grav, thrust, F_w, T_w):
@@ -486,3 +489,208 @@ def test_position_task_runs_unfused(monkeypatch):
         assert torch.isfinite(obs["observations"]).all() and torch.isfinite(rew).all()
         q = task.sim_env.global_tensor_dict["dof_state_tensor"][..., 0]
         assert (q.abs() <= 0.6 + 1e-6).all()
+
+
+# ---- 7. one whole sub-step against the float64 reference ---------------------------------------------------------------------
+# Tolerance of a sub-step's state against AO.substep, derived from the ABA's bar: the float32 ABA is within RTOL of
+# amax = max |(a0, qdd)| of the env (section 2), and the sub-step carries that error through one dt into the velocities (base
+# v, w and qd) and through dt^2 into the positions (base x and quaternion, q); on top comes the float32 rounding of the update
+# itself, at most ULPS ulps of the magnitude of the quantity (its value before or after the sub-step, whichever is larger).
+# Measured worst case over tests/test_zz_articulated_oracle_gpu.py, as a fraction of this tolerance: 0.56 on the host shadow
+# (qd), 0.34 on the H100 (qd; H100 80GB HBM3).
+EPS32 = 2.0 ** -23
+ULPS = 8
+
+
+def shaped_art(rng, B, shape="random", M=4, drive=True, motors="random"):
+    """random_art with the tree's shape and the motors' bodies chosen: shape "chain" (depth B - 1), "star" (every joint on the
+    base) or "random"; motors "base" (all on body 0), "leaves" (round robin over the bodies without children), "cluster" (all but
+    one on the last body) or "random\""""
+    art = random_art(rng, B, drive=drive, M=M)
+    b = art.bodies
+    if shape == "chain":
+        b.parent[1:] = np.arange(B - 1)
+    elif shape == "star":
+        b.parent[1:] = 0
+    leaves = [i for i in range(B) if i not in set(b.parent[1:].tolist())]
+    if motors == "base":
+        art.motor_body[:] = 0
+    elif motors == "leaves":
+        art.motor_body[:] = [leaves[k % len(leaves)] for k in range(M)]
+    elif motors == "cluster":
+        art.motor_body[:] = B - 1
+        art.motor_body[0] = 0
+    return art
+
+
+def substep_inputs(spec, art, N, seed):
+    """seeded inputs of one sub-step (CPU float32 tensors): root, actions, motor constants and gains of _hp1_common.random_inputs,
+    joint state within +-0.8 rad and +-3 rad/s (inside the limits of a limited joint), drive targets, a body-frame disturbance"""
+    root, actions, params = H.random_inputs(spec, N, seed)
+    rng = np.random.default_rng(seed)
+    b, D = art.bodies, art.num_dofs
+    lo = np.where(b.limited[1:], b.lower[1:], -0.8)
+    hi = np.where(b.limited[1:], b.upper[1:], 0.8)
+    q = lo + (hi - lo) * rng.uniform(0.0, 1.0, (N, D))
+    f32 = lambda a: torch.tensor(np.asarray(a, np.float32))
+    return {"root": root, "actions": actions, "params": params, "dof": f32(np.stack([q, rng.uniform(-3, 3, (N, D))], -1)),
+            "qs": f32(rng.uniform(-0.5, 0.5, (N, D))), "qds": f32(rng.uniform(-1, 1, (N, D))),
+            "dist": f32(rng.uniform(-0.3, 0.3, (N, 6)) * [1, 1, 1, 0.01, 0.01, 0.01])}
+
+
+def load_inputs(eng, inp):
+    H.load_engine_state(eng, inp["root"], inp["params"])
+    dev = eng.root_state.device
+    eng.dof_state.copy_(inp["dof"].to(dev))
+    eng.dof_position_setpoint.copy_(inp["qs"].to(dev))
+    eng.dof_velocity_setpoint.copy_(inp["qds"].to(dev))
+
+
+def oracle_state(eng, spec, inp, idx):
+    """hp1_oracle's model and float64 state of envs idx: what the kernel reads -- the per-env arrays the engine holds, the
+    config's float32 constants for the parameters it does not (per_env_params="auto")"""
+    model = H.oracle_model_from_spec(spec)
+    n, M = len(idx), spec.num_motors
+    st = HO.make_state(model, n, torch.float64)
+    st.root, st.thrust = inp["root"][idx].double(), inp["params"]["thrust"][idx].double()
+    for k in ("tau_inc", "tau_dec", "k_thrust", "K_pos", "K_vel", "K_rot", "K_angvel"):
+        if getattr(eng, k) is not None:
+            setattr(st, k, inp["params"][k][idx].double())
+        else:
+            c = getattr(eng.cfg, k)
+            c = [float(c)] * M if k in ("tau_inc", "tau_dec", "k_thrust") else [float(v) for v in c]
+            setattr(st, k, torch.tensor(c, dtype=torch.float64).expand(n, -1).clone())
+    return model, st
+
+
+def reference_substep(eng, spec, art, inp, idx):
+    """AO.substep on envs idx -> (reference dict, well-conditioned mask [len(idx)])"""
+    model, st = oracle_state(eng, spec, inp, idx)
+    ok = H.well_conditioned(model, st, inp["actions"][idx].double()).numpy()
+    dof = inp["dof"][idx].double().numpy()
+    ref = AO.substep(model, table_of(eng.art), st, dof[..., 0], dof[..., 1], inp["qs"][idx].double().numpy(),
+                     inp["qds"][idx].double().numpy(), inp["actions"][idx].double(), inp["dist"][idx].double())
+    return ref, ok
+
+
+def _record(worst, what, err, tol):
+    r = float((err / tol).max()) if err.size else 0.0
+    if worst is not None:
+        worst[what] = max(worst.get(what, (0.0, 0.0)), (r, float(err.max()) if err.size else 0.0))
+    return r
+
+
+LIMIT_BAND = 1e-5  # a reference q' this close to a limit may round to either side of it: the projection may go either way
+
+
+def near_limit(tab, ref):
+    """bool [n]: envs with a limited joint whose unprojected reference q' lies within LIMIT_BAND of one of its limits"""
+    D = int(tab["num_bodies"]) - 1
+    lim = tab["limited"][1:D + 1].astype(bool)
+    lo, hi, qf = tab["lower"][1:D + 1], tab["upper"][1:D + 1], ref["q_free"]
+    return (lim & ((np.abs(qf - lo) < LIMIT_BAND) | (np.abs(qf - hi) < LIMIT_BAND))).any(1)
+
+
+def check_substep(eng, spec, inp, ref, ok, idx, worst=None):
+    """the engine's state after one sub-step (envs idx) against the reference, with the tolerance above.  Envs that fail
+    _hp1_common.well_conditioned, and those near_limit, are only checked for finite values.  worst: a dict that collects
+    (worst err / tol, worst |err|) per quantity.  -> the number of envs left out for a joint near a limit"""
+    dt = spec.dt
+    got = lambda t: t.detach().cpu().double().numpy()[idx]
+    root, dof, thrust = got(eng.root_state), got(eng.dof_state), got(eng.motor_thrust)
+    for t in (root, dof, thrust):
+        assert np.isfinite(t).all()
+    near = near_limit(table_of(eng.art), ref)
+    keep = ok & ~near
+    amax = np.abs(np.concatenate([ref["a0"], ref["qdd"]], 1)).max(1)[keep][:, None]
+    r_in, dof_in = inp["root"][idx].double().numpy()[keep], inp["dof"][idx].double().numpy()[keep]
+    r_ref = ref["root"][keep]
+    mag = lambda *a: np.max([np.abs(x).max(-1, keepdims=True) for x in a], 0)
+    checks = {
+        "x": (root[keep, 0:3], r_ref[:, 0:3], mag(r_ref[:, 0:3], r_in[:, 0:3]) + dt * mag(r_ref[:, 7:10]), 2),
+        "quat": (root[keep, 3:7], r_ref[:, 3:7], 1.0 + dt * mag(r_ref[:, 10:13]), 2),
+        "v": (root[keep, 7:10], r_ref[:, 7:10], mag(r_ref[:, 7:10], r_in[:, 7:10]), 1),
+        "w": (root[keep, 10:13], r_ref[:, 10:13], mag(r_ref[:, 10:13], r_in[:, 10:13]), 1),
+        "q": (dof[keep, :, 0], ref["q"][keep], np.maximum(np.abs(ref["q"][keep]), np.abs(dof_in[..., 0])) + dt * np.abs(ref["qd"][keep]), 2),
+        "qd": (dof[keep, :, 1], ref["qd"][keep], np.maximum(np.abs(ref["qd"][keep]), np.abs(dof_in[..., 1])), 1),
+    }
+    for what, (g, r, m, p) in checks.items():
+        err = np.abs(g - r)
+        tol = ULPS * EPS32 * m + dt ** p * RTOL * amax
+        bad = ~(err <= tol)
+        assert not bad.any(), f"{what}: {bad.sum()}/{bad.size} outside tol, worst err/tol {(err / tol).max():.3g} at env " \
+                              f"{np.asarray(idx)[keep][np.argwhere(bad)[0][0]]}"
+        _record(worst, what, err, tol)
+    fs = max(1.0, float(np.abs(ref["thrust"][ok]).max(initial=0.0)))
+    H.assert_close(thrust[ok], ref["thrust"][ok], "motor_thrust", scale=fs)
+    _record(worst, "thrust", np.abs(thrust[ok] - ref["thrust"][ok]), H.RTOL * np.maximum(np.abs(ref["thrust"][ok]), fs))
+    check_derived(eng, ref["derived"], idx, ok, worst)
+    return int(near.sum())
+
+
+def check_derived(eng, d, idx, ok, worst=None):
+    """the five derived outputs against update_states in float64 (_hp1_common's scales)"""
+    for k, scale in (("euler", math.pi), ("vehicle_orientation", 1.0), ("vehicle_linvel", None), ("body_linvel", None),
+                     ("body_angvel", None)):
+        g = getattr(eng, k).detach().cpu().double().numpy()[idx]
+        assert np.isfinite(g).all(), k
+        g, r = g[ok], d[k][ok]
+        s = scale if scale is not None else max(float(np.abs(r).max(initial=0.0)), 1e-30)
+        H.assert_close(g, r, k, scale=s)
+        _record(worst, k, np.abs(g - r), H.RTOL * np.maximum(np.abs(r), s))
+
+
+def test_substep_reference_reduces_to_hp1_physics_step():
+    """One body, its COM at the base origin, the same mass and inertia as the HP1 model, gyroscopic term on: there the ABA's
+    floating base is the rigid body of DESIGN section 3, and AO.substep must be hp1_oracle.physics_step (float64 both, drag,
+    disturbance, damping and both caps active).  Measured residual: 2.8e-15 absolute, 1.3e-15 relative to the env's state."""
+    n = 256
+    spec = H.spec_for("quad_attitude")
+    spec.drag_lin1, spec.drag_lin2, spec.drag_ang1, spec.drag_ang2 = (0.1, 0.1, 0.2), (0.05, 0.05, 0.1), (1e-3,) * 3, (5e-4,) * 3
+    spec.linear_damping, spec.angular_damping, spec.max_linear_velocity, spec.max_angular_velocity = 0.3, 0.4, 1.5, 2.5
+    model = H.oracle_model_from_spec(spec)
+    assert model.gyroscopic and not model.com.any()
+    # the table in float64 (table_of would round it to the float32 struct): body 0 = the HP1 rigid body, the motors its links
+    z1 = np.zeros(1)
+    tab = {"num_bodies": 1, "parent": np.array([-1]), "joint_R": np.eye(3)[None], "joint_p": np.zeros((1, 3)), "axis": np.zeros((1, 3)),
+           "mass": np.array([model.mass]), "com": np.zeros((1, 3)), "inertia": model.inertia[None], "stiffness": z1, "damping": z1,
+           "motor_body": np.zeros(4, int), "motor_R": model.link_R, "motor_p": model.link_r,
+           "motor_torque": -model.thrust_to_torque_ratio * model.motor_directions, "lower": z1, "upper": z1, "limited": z1}
+    root, actions, params = H.random_inputs(spec, n, 17)
+    st = H.load_oracle_state(model, root.double(), {k: v.double() for k, v in params.items()}, n)
+    st.root[:, 3:7] /= st.root[:, 3:7].norm(dim=1, keepdim=True)  # unit in float64: the two sides rotate by different formulas
+    st.root[:, 7:13] *= 1.5  # most envs start above a cap
+    dist = torch.rand(n, 6, dtype=torch.float64, generator=torch.Generator().manual_seed(2)) - 0.5
+    z = np.zeros((n, 0))
+    ref = AO.substep(model, tab, st.clone(), z, z, z, z, actions.double(), dist)
+    st1 = st.clone()
+    HO.physics_step(model, st1, actions.double(), dist)
+    scale = st1.root.abs().max(dim=1, keepdim=True).values.numpy()
+    assert np.abs(ref["root"] - st1.root.numpy()).max() <= 1e-9 * scale.max()
+    assert (np.abs(ref["root"] - st1.root.numpy()) / scale).max() < 1e-12
+    np.testing.assert_allclose(ref["thrust"], st1.thrust.numpy(), rtol=1e-12, atol=0)
+    for k, v in st1.derived.items():
+        np.testing.assert_array_equal(ref["derived"][k], v.numpy())
+    capped = (st.root[:, 7:10].norm(dim=1) > 1.5) & (torch.from_numpy(ref["root"][:, 7:10]).norm(dim=1) > 1.5 - 1e-9)
+    assert capped.any()
+
+
+@pytest.mark.parametrize("M", [4, 8])
+def test_shadow_substep_matches_reference_on_random_trees(M):
+    """shadow_art_step (one sub-step) against AO.substep on random trees of 1-16 bodies, with the tolerance of section 7"""
+    rng = np.random.default_rng(40 + M)
+    spec = H.spec_for("quad_attitude" if M == 4 else "octa_velocity")
+    worst = {}
+    for trial in range(16):
+        B = trial + 1
+        art = shaped_art(rng, B, M=M, drive=bool(trial % 2))
+        n = 24
+        eng = CpuArticulatedHp1Engine(spec, n, per_env_params="all", articulation=art)
+        inp = substep_inputs(spec, art, n, 100 + trial)
+        load_inputs(eng, inp)
+        eng.physics_step(inp["actions"], disturbance=inp["dist"], physics_steps=1)
+        idx = np.arange(n)
+        ref, ok = reference_substep(eng, spec, art, inp, idx)
+        assert ok.mean() > 0.8
+        check_substep(eng, spec, inp, ref, ok, idx, worst)
+    print({k: f"{v[0]:.2f} ({v[1]:.1e})" for k, v in worst.items()})
