@@ -4,8 +4,8 @@ Articulated robots (ROV, reconfigurable, Morphy) are out of the hot-path scope (
 import numpy as np
 
 from . import RESOURCES_DIRECTORY
-from .sensor_config import (BaseDepthCameraConfig, BaseImuConfig, BaseLidarConfig, BaseNormalFaceIDCameraConfig, OSDome_64_Config,
-                            RSLidar_Airy_Config, StereoCameraConfig, fake_radar_config, pmd_flexx2_config)
+from .sensor_config import (BaseDepthCameraConfig, BaseImuConfig, BaseLidarConfig, BaseNormalFaceIDCameraConfig, GimbalDepthCameraConfig,
+                            OSDome_64_Config, RSLidar_Airy_Config, StereoCameraConfig, fake_radar_config, pmd_flexx2_config)
 
 PI = np.pi
 QUAD_ALLOCATION = [
@@ -471,5 +471,31 @@ class MorphyCompliantCfg(MorphyStiffCfg):
         # uniform reset ranges of the joint state (position rad, velocity rad/s)
         min_init_dof_position = -0.1
         max_init_dof_position = 0.1
+        min_init_dof_velocity = 0.0
+        max_init_dof_velocity = 0.0
+
+
+class BaseQuadWithGimbalCameraCfg(BaseQuadCfg):
+    """base_quadrotor with a two-axis camera gimbal (ours): quad_gimbal.urdf hangs gimbal_roll_joint (about x, +-0.8 rad) ->
+    gimbal_pitch_joint (about y, [-0.8, 1.6] rad, +pi/2 looks straight down) -> gimbal_camera_link 6 cm below the base origin, and
+    the 64 x 48 depth camera rides on gimbal_camera_link.  Each stage is balanced (COM on its axis), so the drive only has to move
+    inertia: the roll subtree has 1.0e-5 kg m^2 about its axis, the pitch stage 6.0e-6.  With k = 0.03 N m / rad the drive's
+    natural frequencies are 55 rad/s (roll) and 71 rad/s (pitch), w dt = 0.55 and 0.71 at dt = 0.01, and d = 7e-4 N m s / rad gives
+    damping ratios of 0.64 and 0.82 (DESIGN.md "Articulated robots").  Targets (-roll, -pitch) of the base's ZYX Euler angles level
+    the camera: Rz(psi) Ry(theta) Rx(phi) Rx(-phi) Ry(-theta) = Rz(psi)."""
+    class sensor_config(BaseQuadCfg.sensor_config):
+        enable_camera = True
+        camera_config = GimbalDepthCameraConfig
+
+    class robot_asset(BaseQuadCfg.robot_asset):
+        file = "quad_gimbal.urdf"
+        name = "base_quadrotor_with_gimbal_camera"
+
+    class joint_config:
+        # per DOF (gimbal_roll_joint, gimbal_pitch_joint); a scalar applies to both
+        stiffness = 0.03
+        damping = 7e-4
+        min_init_dof_position = 0.0
+        max_init_dof_position = 0.0
         min_init_dof_velocity = 0.0
         max_init_dof_velocity = 0.0

@@ -36,6 +36,18 @@ class BaseDepthCameraConfig(BaseSensorConfig):
         pixel_std_dev_multiplier = 0.01
 
 
+class GimbalDepthCameraConfig(BaseDepthCameraConfig):
+    """64 x 48 depth + segmentation camera on gimbal_camera_link of quad_gimbal.urdf (ours): parent_link makes EnvManager take the
+    camera's pose from that link's body row of robot_body_state_tensor; the optical axis is the link's +x; fixed placement."""
+    height, width = 48, 64
+    parent_link = "gimbal_camera_link"
+    randomize_placement = False
+    min_translation = [0.0, 0.0, 0.0]
+    max_translation = [0.0, 0.0, 0.0]
+    min_euler_rotation_deg = [0.0, 0.0, 0.0]
+    max_euler_rotation_deg = [0.0, 0.0, 0.0]
+
+
 class BaseLidarConfig(BaseSensorConfig):
     num_sensors = 1
     sensor_type = "lidar"

@@ -63,7 +63,79 @@ ArtKernel pick_art_kernel(int M, int B) {
     return B <= 9 ? articulated_step_kernel<8, 9> : articulated_step_kernel<8, AGX_ART_MAX_BODIES>;
 }
 
+// ---- per-body state (agx_hp1_articulated_body_state) ----------------------------------------------------------------------
+// One env per lane, one warp per block.  Each lane builds its env's B rows (13 B floats) in shared memory with art_body_states, the
+// rows of the parents serving as the sweep's scratch, so nothing goes to local memory.  Written straight from the lanes, the rows
+// of a warp would sit 52 B apart per lane and no store would coalesce; instead the warp copies its contiguous span of body_state
+// (32 x 13 B floats) out of shared memory with 16-byte stores.  A lane's row in shared memory is 13 B floats, plus one when 13 B is
+// even, so that the 32 lanes' accesses at the same offset fall in 32 different banks.
+constexpr int kBodyThreads = 32;
+
+template <int NB>
+__global__ void __launch_bounds__(kBodyThreads)
+articulated_body_state_kernel(const __grid_constant__ AgxArticulation art, int num_envs, const float* __restrict__ root_state,
+                              int root_stride, float* __restrict__ body_state) {
+    extern __shared__ float4 s_body_rows4[];
+    float* s_rows = reinterpret_cast<float*>(s_body_rows4);
+    const int B = art.num_bodies, D = art.num_dofs;
+    const int len = 13 * B, pad = (len & 1) ^ 1;  // floats of one env's rows; the padding that makes the lane stride odd
+    const int lane = threadIdx.x;
+    const int env0 = blockIdx.x * kBodyThreads;
+    const int env = env0 + lane;
+    if (env < num_envs)
+        art_body_states<NB>(art, root_state + (size_t)env * root_stride, art.dof_state + (size_t)env * 2 * D, s_rows + lane * (len + pad));
+    __syncwarp();
+    const int total = min(kBodyThreads, num_envs - env0) * len;  // floats of the warp's span
+    float* out = body_state + (size_t)env0 * len;               // 16-byte aligned: env0 * len is a multiple of 32 * 13
+    const int n4 = total >> 2;
+    if (pad == 0) {
+        for (int k = lane; k < n4; k += kBodyThreads) reinterpret_cast<float4*>(out)[k] = s_body_rows4[k];
+    } else {
+        for (int k = lane; k < n4; k += kBodyThreads) {
+            const int g = 4 * k, l0 = g / len;
+            float v[4];
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int gj = g + j;
+                v[j] = s_rows[gj + l0 + (gj - l0 * len >= len ? 1 : 0)];  // + (env of float gj) x pad, pad = 1
+            }
+            reinterpret_cast<float4*>(out)[k] = make_float4(v[0], v[1], v[2], v[3]);
+        }
+    }
+    for (int g = 4 * n4 + lane; g < total; g += kBodyThreads) out[g] = s_rows[g + (g / len) * pad];
+}
+
+int validate_body_state(const AgxArticulation* art, int num_envs, const float* root_state, int root_state_stride, const float* body_state) {
+    if (!art) return agx_set_error(AGX_E_NULL, "art is NULL");
+    if (num_envs < 0) return agx_set_error(AGX_E_INVALID, "num_envs < 0");
+    const int B = art->num_bodies;
+    if (B < 1 || B > AGX_ART_MAX_BODIES)
+        return agx_set_error(AGX_E_INVALID, "num_bodies must be in [1, %d] (got %d)", AGX_ART_MAX_BODIES, B);
+    if (art->num_dofs != B - 1) return agx_set_error(AGX_E_INVALID, "num_dofs must be num_bodies - 1");
+    for (int i = 1; i < B; ++i)
+        if (art->parent[i] < 0 || art->parent[i] >= i) return agx_set_error(AGX_E_INVALID, "parent[%d] must be in [0, %d)", i, i);
+    if (root_state_stride < 13) return agx_set_error(AGX_E_INVALID, "root_state_stride < 13");
+    if (num_envs == 0) return AGX_OK;
+    if (!root_state || !body_state) return agx_set_error(AGX_E_NULL, "root_state/body_state is NULL");
+    if (B > 1 && !art->dof_state) return agx_set_error(AGX_E_NULL, "dof_state is NULL");
+    if ((uintptr_t)body_state & 15) return agx_set_error(AGX_E_INVALID, "body_state must be 16-byte aligned");
+    return AGX_OK;
+}
+
 }  // namespace
+
+extern "C" int agx_hp1_articulated_body_state(const AgxArticulation* art, int num_envs, const float* root_state, int root_state_stride,
+                                              float* body_state, void* stream) {
+    int rc = validate_body_state(art, num_envs, root_state, root_state_stride, body_state);
+    if (rc) return rc;
+    if (num_envs == 0) return AGX_OK;
+    const int g = (num_envs + kBodyThreads - 1) / kBodyThreads;
+    const int len = 13 * art->num_bodies;
+    const size_t smem = sizeof(float) * kBodyThreads * (len + ((len & 1) ^ 1));  // <= 26.75 KB at 16 bodies
+    auto kern = art->num_bodies <= 9 ? articulated_body_state_kernel<9> : articulated_body_state_kernel<AGX_ART_MAX_BODIES>;
+    kern<<<g, kBodyThreads, smem, (cudaStream_t)stream>>>(*art, num_envs, root_state, root_state_stride, body_state);
+    return agx_check_launch("articulated_body_state_kernel");
+}
 
 extern "C" int agx_hp1_articulated_step(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, const AgxArticulation* art, void* stream) {
     int rc = validate_articulation(cfg, buf, art);

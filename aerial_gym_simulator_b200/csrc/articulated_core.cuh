@@ -377,4 +377,51 @@ AGX_DEV void art_env_step(const AgxHp1Config& cfg, const AgxHp1Buffers& buf, con
     st3(buf.body_angvel, d.wb);
 }
 
+// ---- per-body state of one env (agx_hp1_articulated_body_state) ------------------------------------------------------------
+// rows [B][13]: body i's row at rows + 13 i, laid out like a root_state row (world position of the body-frame origin, xyzw quaternion
+// body -> world, world linear velocity of the body-frame origin, world angular velocity).  root [13] = the env's root_state row, dof
+// [D][2] = its (q, q-dot).  Row 0 is the root row, copied.  The forward kinematics are art_dynamics': R_i = R_l joint_R_i
+// axis_angle(axis_i, q), P_i = P_l + R_l joint_p_i, V_i = V_l + S_i q-dot with S_i = (a, P_i x a), a = R_l joint_R_i axis_i.  The
+// rows double as the scratch of the sweep (parent before child): while it runs, row i >= 1 holds (P_i relative to the base origin,
+// quaternion of R_i, linear part of V_i = the velocity of the body point at the base origin, w_i), and R_l is rebuilt from row l's
+// quaternion.  A last pass turns each row into world position x_0 + P_i and origin velocity V_lin + w_i x P_i.
+template <int NB>
+AGX_DEV void art_body_states(const AgxArticulation& art, const float* root, const float* dof, float* rows) {
+    const int B = art.num_bodies;
+#pragma unroll
+    for (int k = 0; k < 13; ++k) rows[k] = root[k];
+    for (int i = 1; i < NB; ++i) {
+        if (i >= B) break;
+        // the joint rotation first, while little else is live: sincosf's rarely taken wide-argument reduction then keeps its
+        // six-word table in registers instead of a stack frame
+        const V3 ax = ld3(art.axis[i]);
+        const M33 Rq = axis_angle(ax, dof[2 * (i - 1)]);
+        const int l = art.parent[i];
+        const float* pl = rows + 13 * l;
+        const M33 Rl = quat_to_matrix(Q4{pl[3], pl[4], pl[5], pl[6]});
+        const V3 Pl = (l == 0) ? V3{0.0f, 0.0f, 0.0f} : ld3(pl);
+        const M33 RJ = mul33(Rl, ld33(art.joint_R[i]));
+        const M33 Ri = mul33(RJ, Rq);
+        const V3 Pi = Pl + mul33v(Rl, ld3(art.joint_p[i]));
+        const V3 aw = mul33v(RJ, ax);
+        const V3 lin = cross(Pi, aw);
+        const float qd = dof[2 * (i - 1) + 1];
+        const Q4 qi = matrix_cols_to_quat(V3{Ri.m[0], Ri.m[3], Ri.m[6]}, V3{Ri.m[1], Ri.m[4], Ri.m[7]}, V3{Ri.m[2], Ri.m[5], Ri.m[8]});
+        float* r = rows + 13 * i;
+        r[0] = Pi.x; r[1] = Pi.y; r[2] = Pi.z;
+        r[3] = qi.x; r[4] = qi.y; r[5] = qi.z; r[6] = qi.w;
+        r[7] = pl[7] + lin.x * qd; r[8] = pl[8] + lin.y * qd; r[9] = pl[9] + lin.z * qd;
+        r[10] = pl[10] + aw.x * qd; r[11] = pl[11] + aw.y * qd; r[12] = pl[12] + aw.z * qd;
+    }
+    const V3 x0 = ld3(rows);
+    for (int i = 1; i < NB; ++i) {
+        if (i >= B) break;
+        float* r = rows + 13 * i;
+        const V3 P = ld3(r);
+        const V3 v = ld3(r + 7) + cross(ld3(r + 10), P);
+        r[0] = x0.x + P.x; r[1] = x0.y + P.y; r[2] = x0.z + P.z;
+        r[7] = v.x; r[8] = v.y; r[9] = v.z;
+    }
+}
+
 }  // namespace agx

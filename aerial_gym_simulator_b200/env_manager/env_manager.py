@@ -66,6 +66,27 @@ def _quat_from_euler(e):  # utils/math.py:155-172
                         cy * cr * cp + sy * sr * sp], dim=-1)
 
 
+def _quat_mul(a, b):  # xyzw Hamilton product
+    ax, ay, az, aw = a.unbind(-1)
+    bx, by, bz, bw = b.unbind(-1)
+    return torch.stack([aw * bx + bw * ax + ay * bz - az * by, aw * by + bw * ay + az * bx - ax * bz,
+                        aw * bz + bw * az + ax * by - ay * bx, aw * bw - ax * bx - ay * by - az * bz], dim=-1)
+
+
+def _matrix_to_quat(R):
+    """xyzw quaternion of a rotation matrix (Shepperd's method, float64)"""
+    t = np.trace(R)
+    if t > 0:
+        s = 2.0 * np.sqrt(1.0 + t)
+        return np.array([(R[2, 1] - R[1, 2]) / s, (R[0, 2] - R[2, 0]) / s, (R[1, 0] - R[0, 1]) / s, 0.25 * s])
+    i = int(np.argmax(np.diag(R)))
+    j, k = (i + 1) % 3, (i + 2) % 3
+    s = 2.0 * np.sqrt(1.0 + R[i, i] - R[j, j] - R[k, k])
+    v = np.zeros(4)
+    v[i], v[j], v[k], v[3] = 0.25 * s, (R[j, i] + R[i, j]) / s, (R[k, i] + R[i, k]) / s, (R[k, j] - R[j, k]) / s
+    return v
+
+
 def _obstacle_mass_row(model, path):
     """the AgxObstacleMass row of a free obstacle asset: the composite mass properties of its URDF inertials (the robot's come from
     the same function).  No density is assumed: an asset without mass is an error."""
@@ -217,6 +238,11 @@ class EnvManager:
             gtd["dof_velocity_setpoint_tensor"] = eng.dof_velocity_setpoint
             T = lambda v: torch.tensor(np.asarray(v, np.float32), device=dev)
             self._dof_rng = tuple(T(r) for r in (*articulation.init_dof_pos_range, *articulation.init_dof_vel_range))
+        # every body's pose and velocity [N,B,13] (rows like robot_state_tensor's, body 0 = the root link), refreshed once per env step
+        self._body_state = getattr(eng, "body_state", None) if articulation is not None else None
+        if self._body_state is not None:
+            gtd["robot_body_state_tensor"] = self._body_state
+            gtd["robot_body_names"] = list(articulation.bodies.links)
         self.robot.controller.bind_engine(eng)  # controller.K_*_tensor_current / set_controller_gains act on the engine's gains
         gtd["crashes"], gtd["truncations"] = eng.terminations, eng.truncations
         self.collision_tensor, self.truncation_tensor = eng.terminations, eng.truncations
@@ -250,6 +276,7 @@ class EnvManager:
         eng.bounds_max.copy_(_lerp(self._bounds_rng[2], self._bounds_rng[3], torch.rand(N, 3, device=dev)))
         self._build_obstacles()
         self._build_sensors()
+        self._update_body_state()  # the rows of the creation pose, until the first reset
         if eng.host_io and (self.scene is not None or self.reset_rng != "device" or self.contact_mode == "rigid"):
             raise NotImplementedError("args['host_io'] needs an obstacle-free env, reset_rng='device' and contact='flag': the flags "
                                       "live in host memory and are written only by the fused task step")
@@ -431,7 +458,7 @@ class EnvManager:
     def _build_sensors(self):
         gtd, N, dev = self.global_tensor_dict, self.num_envs, self.device
         sc = self.robot_cfg.sensor_config
-        self.sensor, self.sensor_cfg = None, None
+        self.sensor, self.sensor_cfg, self._sensor_link = None, None, None
         self.imu = None
         if getattr(sc, "enable_imu", False):  # robot_manager.py:91-96, 246-262
             from ..sensors import IMUSensor
@@ -462,9 +489,24 @@ class EnvManager:
         self.sensor_mount = torch.zeros(N, S, 7, device=dev)
         mean_e = (self._mount_rng[2] + self._mount_rng[3]) / 2.0  # warp_sensor.py:118-123
         self.sensor_mount[..., 3:7] = _quat_from_euler(mean_e.expand(N, S, 3))
-        self.sensor = RaySensor(cfg, self.scene, self.engine.root_state, gtd["depth_range_pixels"], seg, self.sensor_mount)
-        self.sensor.mount = self.sensor_mount  # keep the live tensor (RaySensor made it contiguous already)
-        self.sensor.c.mount = self.sensor_mount.data_ptr()
+        # a sensor on a link (cfg.parent_link): pose = body pose o T_l o mount o frame rotation.  The cast reads the link's body row
+        # of robot_body_state_tensor (robot_state_tensor on a robot without joints) and a mount with T_l folded in; sensor_mount
+        # stays relative to the link
+        pose, mount = self.engine.root_state, self.sensor_mount
+        link = getattr(cfg, "parent_link", None)
+        if link is not None:
+            b, R_l, p_l = self._resolve_link(link)
+            if self._body_state is not None:
+                pose = self._body_state[:, b, :]
+            elif b != 0:
+                raise ValueError(f"sensor parent_link '{link}' moves with a joint, and the engine publishes no per-body state")
+            T = lambda v: torch.tensor(np.asarray(v, np.float32), device=dev)
+            self._sensor_link = (T(R_l), T(p_l), T(_matrix_to_quat(np.asarray(R_l, np.float64))))
+            mount = self.sensor_mount_body = torch.zeros(N, S, 7, device=dev)
+            self._fold_link_into_mount()
+        self.sensor = RaySensor(cfg, self.scene, pose, gtd["depth_range_pixels"], seg, mount)
+        self.sensor.mount = mount  # keep the live tensor (RaySensor made it contiguous already)
+        self.sensor.c.mount = mount.data_ptr()
         # sensor noise (WarpSensor.apply_noise, warp_sensor.py:227-250): "device" = one in-place pass with a counter-based
         # device RNG (agx_hp2_noise_limits; default next to the in-kernel Philox resets), "torch" = the reference's torch calls
         # in the reference's order (default when reset_rng == "torch", i.e. when every random number comes from torch)
@@ -478,6 +520,25 @@ class EnvManager:
             per_env = px[0].numel() // (3 if pc else 1)
             self._device_noise = DeviceSensorNoise(cfg, px, seed=int(self.env_args.get("seed", 0)) ^ 0x5E4503_4E015E,
                                                    first_pixel=int(self.env_args.get("env_id_offset", 0)) * per_env)
+
+    def _resolve_link(self, name):
+        """(body, R_l, p_l): the body a URDF link belongs to and the link's frame in that body's frame (on a robot without joints:
+        body 0 and the link's fixed transform from the root link)"""
+        model = self.robot.urdf_model
+        if name not in model.links:
+            raise ValueError(f"sensor parent_link '{name}' is not a link of robot '{self.robot_name}'; its links are {sorted(model.links)}")
+        if self.articulated:
+            R, p = self.robot.bodies.link_in_body[name]
+            return self.robot.bodies.link_body[name], R, p
+        R, p = model.link_transforms()[name]
+        return 0, R, p
+
+    def _fold_link_into_mount(self):
+        """sensor_mount_body = T_l o sensor_mount (position p_l + R_l m_p, orientation q_l (x) m_q), after every mount draw"""
+        R, p, q = self._sensor_link
+        m = self.sensor_mount
+        self.sensor_mount_body[..., 0:3] = p + (R * m[..., None, 0:3]).sum(-1)
+        self.sensor_mount_body[..., 3:7] = _quat_mul(q.expand_as(m[..., 3:7]), m[..., 3:7])
 
     # ------------------------------------------------------------------------------------------
     # reset (env_manager.py:273-301)
@@ -553,9 +614,16 @@ class EnvManager:
             t0, t1, e0, e1 = self._mount_rng
             self.sensor_mount[env_ids, :, 0:3] = _lerp(t0, t1, torch.rand(k, S, 3, device=dev))
             self.sensor_mount[env_ids, :, 3:7] = _quat_from_euler(_lerp(e0, e1, torch.rand(k, S, 3, device=dev)))
+        if self.sensor is not None and self._sensor_link is not None:
+            self._fold_link_into_mount()
         if self.imu is not None:
             self.imu.reset_idx(env_ids)
         eng.refresh()  # update_states of ALL envs (base_multirotor.py:204-205); sim_steps zeroed by the kernel
+        self._update_body_state()
+
+    def _update_body_state(self):
+        if self._body_state is not None:
+            self.engine.update_body_state()
 
     def _sample_assets_and_update_scene(self, env_ids, mask, A):
         gtd, dev = self.global_tensor_dict, self.device
@@ -724,6 +792,7 @@ class EnvManager:
             self.engine.physics_step(a, physics_steps=n)  # n sub-steps fused in one launch
         if obstacles_move and not moving and n > 0:  # ObstacleManager.pre_physics_step, obstacle_manager.py:40-44
             self._step_obstacles(gtd["env_actions"], n)
+        self._update_body_state()
         self.engine.sim_steps += 1
         self.step_counter += 1
 
@@ -736,6 +805,7 @@ class EnvManager:
         self.engine.physics_step(gtd["robot_actions"], disturbance=self._draw_disturbance(), physics_steps=1)
         if env_actions is not None and self.num_obs_in_env > 1:
             self._step_obstacles(env_actions, 1)
+        self._update_body_state()
 
     def render_viewer(self):
         return None  # headless by construction: there is no Isaac Gym viewer (env_manager.py:389-391)

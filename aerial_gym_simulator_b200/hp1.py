@@ -280,7 +280,8 @@ class Hp1Engine:
         reads in place.  The caller synchronises the stream before reading the results.
         articulation: an ArticulationSpec -- the robot has joints; physics_step runs agx_hp1_articulated_step and the engine owns
         dof_state [N,D,2] and the drive targets dof_position_setpoint / dof_velocity_setpoint [N,D] (zero until the caller writes
-        them).  There is no fused task step for such a robot."""
+        them), and body_state [N,B,13], every body's pose and velocity, which update_body_state() refreshes.  There is no fused task
+        step for such a robot."""
         self.lib = _lib.load()
         self.device = torch.device(device)
         if self.device.type != "cuda":
@@ -291,6 +292,7 @@ class Hp1Engine:
                                 seed=seed, env_id_offset=env_id_offset, device_rng_reset=device_rng_reset,
                                 strict_stale_obs=strict_stale_obs)
         N, M, dev = self.N, self.M, self.device
+        self._init_body_state()
         z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=dev)
         self.root_state = z(N, 13)
         self.root_state[:, 6] = 1.0
@@ -368,6 +370,13 @@ class Hp1Engine:
         self.art.dof_position_setpoint = self.dof_position_setpoint.data_ptr()
         self.art.dof_velocity_setpoint = self.dof_velocity_setpoint.data_ptr()
         self._art_ref = C.byref(self.art)
+
+    def _init_body_state(self):
+        """body_state [N,B,13] of an articulated robot (None otherwise), zero until update_body_state()"""
+        self.body_state = None
+        if self.articulation is not None:
+            B = self.articulation.bodies.num_bodies
+            self.body_state = torch.zeros(self.N, B, 13, dtype=torch.float32, device=self.device)
 
     def _host_tensor(self, shape, dtype):
         nbytes = max(1, int(np.prod(shape))) * torch.empty((), dtype=dtype).element_size()
@@ -504,6 +513,15 @@ class Hp1Engine:
                        "agx_hp1_articulated_step")
             return
         _lib.check(self.lib.agx_hp1_physics_step(self._cfg_ref, self._buf_ref, self._stream()), "agx_hp1_physics_step")
+
+    def update_body_state(self):
+        """body_state [N,B,13] of an articulated robot from root_state and dof_state (agx_hp1_articulated_body_state): per body the
+        world position of its frame origin, the xyzw quaternion body -> world, the world linear velocity of the origin and the world
+        angular velocity; row 0 is root_state's.  One launch, no RNG, capturable."""
+        if self.art is None:
+            raise ValueError("body_state belongs to an articulated robot (Hp1Engine(articulation=...))")
+        _lib.check(self.lib.agx_hp1_articulated_body_state(self._art_ref, self.N, self.root_state.data_ptr(), self.root_state.stride(0),
+                                                           self.body_state.data_ptr(), self._stream()), "agx_hp1_articulated_body_state")
 
     def position_task_step(self, actions, disturbance=None, physics_steps=None, mid_event=None):
         """mid_event: optional torch.cuda.Event(enable_timing=True), already recorded once (so its

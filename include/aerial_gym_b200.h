@@ -264,6 +264,17 @@ typedef struct AgxArticulation {
  * allocation, no synchronisation. */
 int agx_hp1_articulated_step(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, const AgxArticulation* art, void* stream);
 
+/* Pose and velocity of every body of an articulated robot, from the root state and art->dof_state (the other [N,...] arrays of
+ * `art` are not read).  root_state [N,stride] (stride >= 13, rows as AgxHp1Buffers.root_state); body_state [N,B,13] out, dense,
+ * 16-byte aligned, bodies in table order, each row laid out like a root_state row:
+ *   world position of the body-frame origin (3), xyzw quaternion body frame -> world (4; its sign is not normalised),
+ *   world linear velocity of the body-frame origin (3), world angular velocity (3).
+ * Row 0 is the root_state row, copied bit for bit.  Forward kinematics as agx_hp1_articulated_step's: R_i = R_parent joint_R_i
+ * Rot(axis_i, q_i), P_i = P_parent + R_parent joint_p_i, velocities through the joints' motion subspaces.  Capturable: no RNG, no
+ * allocation, no synchronisation. */
+int agx_hp1_articulated_body_state(const AgxArticulation* art, int num_envs, const float* root_state, int root_state_stride,
+                                   float* body_state, void* stream);
+
 /* Masked re-initialisation, EnvManager.reset_idx for a robot-only scene
  * (env_manager/env_manager.py:273-301 -> IGE_env_manager.py:513-519, base_multirotor.py:177-205,
  * base_lee_controller.py:101-118, motor_model.py:140-154).  `mask` [N] bool selects envs.
