@@ -781,7 +781,7 @@ inline int coop_capacity(StepKernel k) {
 // resident after its ready gate has seen the step published, so the push CTAs themselves (256 threads each: 24 of them take the
 // threads of 96 step CTAs) need not fit beside the step.  32 is that bound for a ring of 4 plus margin; the margin is not measured on
 // multi-GPU H100s.  H100: 132 SMs x 8 = 1056 slots - 32 = 1024 = exactly the grid of 65,536 envs.  Any loss of occupancy or fewer
-// SMs moves that size to the two-launch path (same results, slower): bench.py's config5_env_sweep reports the path per size.
+// SMs moves that size to the two-launch path (slower; same results except roll / yaw after a reset, DESIGN §6 Checks): bench.py's config5_env_sweep reports the path per size.
 #ifndef AGX_HP1_COOP_RESERVE
 #define AGX_HP1_COOP_RESERVE 32
 #endif
