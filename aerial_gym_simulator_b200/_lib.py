@@ -156,6 +156,13 @@ class AgxObstacleHull(C.Structure):
                 ("num_files", C.c_int32)]
 
 
+class AgxObstacleBoxes(C.Structure):
+    _fields_ = [("boxes", C.c_void_p), ("asset_file", C.c_void_p), ("num_files", C.c_int32)]
+
+
+OBSTACLE_MAX_ASSETS, OBSTACLE_MAX_CONTACTS = 64, 128  # AGX_OBSTACLE_MAX_ASSETS, AGX_OBSTACLE_MAX_CONTACTS
+
+
 ART_MAX_BODIES = 16  # AGX_ART_MAX_BODIES
 
 
@@ -250,6 +257,8 @@ def load():
                                     C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
         "agx_obstacle_ground_contact": [C.c_int, C.c_int, C.POINTER(AgxContactParams), C.c_void_p, C.c_int, C.c_void_p,
                                         C.POINTER(AgxObstacleHull), C.c_void_p],
+        "agx_obstacle_obstacle_contact": [C.c_int, C.c_int, C.POINTER(AgxContactParams), C.c_void_p, C.c_int, C.c_void_p,
+                                          C.POINTER(AgxObstacleBoxes), C.c_void_p],
     }.items():
         try:
             fn = getattr(lib, name)
@@ -266,7 +275,7 @@ def load():
             or lib.agx_sizeof(7) != C.sizeof(AgxLidarNavRewardParams) or lib.agx_sizeof(8) != C.sizeof(AgxHp2Noise) \
             or lib.agx_sizeof(9) != C.sizeof(AgxE2ERewardParams) or lib.agx_sizeof(11) != C.sizeof(AgxContactParams) \
             or lib.agx_sizeof(12) != C.sizeof(AgxContactMotion) or lib.agx_sizeof(13) != C.sizeof(AgxObstacleMass) \
-            or lib.agx_sizeof(14) != C.sizeof(AgxObstacleHull):
+            or lib.agx_sizeof(14) != C.sizeof(AgxObstacleHull) or lib.agx_sizeof(16) != C.sizeof(AgxObstacleBoxes):
         raise AgxError("aux ABI struct size mismatch between _lib.py and libaerial_gym_b200.so")
     if lib.agx_sizeof(0) != C.sizeof(AgxHp1Config) or lib.agx_sizeof(1) != C.sizeof(AgxHp1Buffers) \
             or lib.agx_sizeof(2) != C.sizeof(AgxHp1ResetDraws) or lib.agx_sizeof(10) != C.sizeof(AgxObsGatherPush) \

@@ -65,6 +65,7 @@ uint64_t agx_sizeof(int which) {
         case 12: return sizeof(AgxContactMotion);
         case 13: return sizeof(AgxObstacleMass);
         case 14: return sizeof(AgxObstacleHull);
+        case 16: return sizeof(AgxObstacleBoxes);
 #endif
         default: return 0;
     }

@@ -478,4 +478,293 @@ AGX_DEV int obstacle_ground_row(const AgxContactParams& P, float* row, const Agx
     return n;
 }
 
+// ---- Obstacle-obstacle contact of free obstacles (agx_obstacle_obstacle_contact; DESIGN.md "Contact between free obstacles").
+// Every asset is one oriented box.  box [15] (asset frame, AgxObstacleBoxes): centre, the three unit axes, the half extents.
+
+// an asset's box in the world: centre c, axes a[3k..3k+2] (axis k), half extents h, bounding-sphere radius r = |h|
+struct ObstacleBox {
+    float c[3], a[9], h[3], r;
+};
+
+AGX_DEV void obstacle_box_world(const float* row, const float* box, ObstacleBox& b) {
+    float R[9], t[3];
+    cquat_R(row + 3, R);
+    cmatvec(R, box, t);
+    for (int k = 0; k < 3; ++k) b.c[k] = row[k] + t[k];
+    for (int k = 0; k < 3; ++k) cmatvec(R, box + 3 + 3 * k, b.a + 3 * k);
+    for (int k = 0; k < 3; ++k) b.h[k] = box[12 + k];
+    b.r = sqrtf(cdot(b.h, b.h));
+}
+
+// broad phase: the bounding spheres are within contact_offset of each other
+AGX_DEV bool obstacle_box_near(const AgxContactParams& P, const ObstacleBox& A, const ObstacleBox& B) {
+    float d[3];
+    for (int k = 0; k < 3; ++k) d[k] = B.c[k] - A.c[k];
+    const float s = A.r + B.r + P.contact_offset;
+    return cdot(d, d) <= s * s;
+}
+
+// separation of the two boxes along the unit axis L (d = B.c - A.c): |d.L| - (sum_k hA_k |a_k.L| + sum_k hB_k |b_k.L|)
+AGX_DEV float obb_sep(const ObstacleBox& A, const ObstacleBox& B, const float* d, const float* L) {
+    float rA = 0.0f, rB = 0.0f;
+    for (int k = 0; k < 3; ++k) {
+        rA = rA + A.h[k] * fabsf(cdot(A.a + 3 * k, L));
+        rB = rB + B.h[k] * fabsf(cdot(B.a + 3 * k, L));
+    }
+    return fabsf(cdot(d, L)) - (rA + rB);
+}
+
+// Narrow phase of one pair: the separating-axis test on the 15 axes (faces of A, faces of B, a_i x b_j with i outer), and the
+// contact manifold.  A pair with any axis separated by more than contact_offset has no contact.  Axis choice, largest separation
+// (least penetration) with a bias, first in axis order on ties: B's face only if it beats A's by more than AGX_OBB_AXIS_TOL, an edge
+// pair only if it beats both faces by more than AGX_OBB_AXIS_TOL; edge axes with |a_i x b_j|^2 < 1e-6 (near-parallel edges) are
+// skipped.  Normal n: the chosen axis, pointing from A to B.
+// Face axis: the incident face (of the other box, the one most anti-parallel to the reference face's outward normal, first axis on
+// ties) is clipped against the reference face's four side planes; every clipped point whose separation s along the outward normal
+// is <= contact_offset is a contact at the incident point moved s / 2 towards the reference face, depth -s.  Edge axis: one contact
+// at the midpoint of the closest points of the two edges (each clamped to its edge), depth = -separation.  At most AGX_CONTACT_MAX
+// (= 8, the most a clipped quad can have) are kept, ordered by contact_insert on the key s: deepest first, ties to the lower index
+// in the clipped polygon.  c [AGX_CONTACT_MAX] gets them (normal from A to B); returns their number.
+#define AGX_OBB_AXIS_TOL 1e-4f
+AGX_DEV int obstacle_box_pair(const AgxContactParams& P, const ObstacleBox& A, const ObstacleBox& B, ContactPt* c) {
+    float d[3];
+    for (int k = 0; k < 3; ++k) d[k] = B.c[k] - A.c[k];
+    const float co = P.contact_offset;
+    float sA = 0.0f, sB = 0.0f, sE = 0.0f;
+    int kA = 0, kB = 0, kE = -1;
+    for (int k = 0; k < 3; ++k) {
+        const float s = obb_sep(A, B, d, A.a + 3 * k);
+        if (s > co) return 0;
+        if (k == 0 || s > sA) {
+            sA = s;
+            kA = k;
+        }
+    }
+    for (int k = 0; k < 3; ++k) {
+        const float s = obb_sep(A, B, d, B.a + 3 * k);
+        if (s > co) return 0;
+        if (k == 0 || s > sB) {
+            sB = s;
+            kB = k;
+        }
+    }
+    float LE[3] = {0.0f, 0.0f, 0.0f};
+    for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) {
+            float L[3];
+            ccross(A.a + 3 * i, B.a + 3 * j, L);
+            const float l2 = cdot(L, L);
+            if (l2 < 1e-6f) continue;
+            const float inv = 1.0f / sqrtf(l2);
+            for (int k = 0; k < 3; ++k) L[k] = L[k] * inv;
+            const float s = obb_sep(A, B, d, L);
+            if (s > co) return 0;
+            if (kE < 0 || s > sE) {
+                sE = s;
+                kE = 3 * i + j;
+                for (int k = 0; k < 3; ++k) LE[k] = L[k];
+            }
+        }
+    const bool refB = sB > sA + AGX_OBB_AXIS_TOL;
+    const float sF = refB ? sB : sA;
+    float n[3];
+    if (kE >= 0 && sE > sF + AGX_OBB_AXIS_TOL) {
+        // edge a_i against edge b_j
+        const int i = kE / 3, j = kE % 3;
+        const float sg = cdot(d, LE) >= 0.0f ? 1.0f : -1.0f;
+        for (int k = 0; k < 3; ++k) n[k] = LE[k] * sg;
+        float pa[3], pb[3];
+        for (int k = 0; k < 3; ++k) {
+            pa[k] = A.c[k];
+            pb[k] = B.c[k];
+        }
+        for (int m = 0; m < 3; ++m) {
+            if (m != i) {
+                const float s = cdot(A.a + 3 * m, n) >= 0.0f ? A.h[m] : -A.h[m];
+                for (int k = 0; k < 3; ++k) pa[k] = pa[k] + A.a[3 * m + k] * s;
+            }
+            if (m != j) {
+                const float s = cdot(B.a + 3 * m, n) > 0.0f ? -B.h[m] : B.h[m];
+                for (int k = 0; k < 3; ++k) pb[k] = pb[k] + B.a[3 * m + k] * s;
+            }
+        }
+        const float* da = A.a + 3 * i;
+        const float* db = B.a + 3 * j;
+        float w[3];
+        for (int k = 0; k < 3; ++k) w[k] = pa[k] - pb[k];
+        const float b = cdot(da, db), dd = cdot(da, w), e = cdot(db, w);
+        const float den = 1.0f - b * b;
+        const float ta = fminf(fmaxf((b * e - dd) / den, -A.h[i]), A.h[i]);
+        const float tb = fminf(fmaxf((e - b * dd) / den, -B.h[j]), B.h[j]);
+        for (int k = 0; k < 3; ++k) c[0].p[k] = ((pa[k] + da[k] * ta) + (pb[k] + db[k] * tb)) * 0.5f;
+        for (int k = 0; k < 3; ++k) c[0].n[k] = n[k];
+        c[0].depth = -sE;
+        return 1;
+    }
+    // face: reference box R (face axis kr, outward normal nr towards the other box), incident box I
+    const ObstacleBox& R = refB ? B : A;
+    const ObstacleBox& I = refB ? A : B;
+    const int kr = refB ? kB : kA;
+    {
+        const float sg = cdot(d, R.a + 3 * kr) >= 0.0f ? 1.0f : -1.0f;
+        for (int k = 0; k < 3; ++k) n[k] = R.a[3 * kr + k] * sg;  // from A to B
+    }
+    float nr[3], fc[3];
+    for (int k = 0; k < 3; ++k) nr[k] = refB ? -n[k] : n[k];
+    for (int k = 0; k < 3; ++k) fc[k] = R.c[k] + nr[k] * R.h[kr];
+    const int r1 = (kr + 1) % 3, r2 = (kr + 2) % 3;
+    const float* t1 = R.a + 3 * r1;
+    const float* t2 = R.a + 3 * r2;
+    const float e1 = R.h[r1], e2 = R.h[r2];
+    int m = 0;
+    float best = fabsf(cdot(nr, I.a));
+    for (int k = 1; k < 3; ++k) {
+        const float v = fabsf(cdot(nr, I.a + 3 * k));
+        if (v > best) {
+            best = v;
+            m = k;
+        }
+    }
+    const float so = cdot(nr, I.a + 3 * m) > 0.0f ? -I.h[m] : I.h[m];
+    const int u = (m + 1) % 3, v = (m + 2) % 3;
+    // the incident face's corners in the reference frame (x along t1, y along t2, s along nr from the reference face)
+    float poly[2][AGX_CONTACT_MAX][3];
+    int np = 4;
+    const float su[4] = {1.0f, -1.0f, -1.0f, 1.0f}, sv[4] = {1.0f, 1.0f, -1.0f, -1.0f};
+    for (int q = 0; q < 4; ++q) {
+        float rel[3];
+        for (int k = 0; k < 3; ++k)
+            rel[k] = ((I.c[k] + I.a[3 * m + k] * so) + I.a[3 * u + k] * (su[q] * I.h[u]) + I.a[3 * v + k] * (sv[q] * I.h[v])) - fc[k];
+        poly[0][q][0] = cdot(rel, t1);
+        poly[0][q][1] = cdot(rel, t2);
+        poly[0][q][2] = cdot(rel, nr);
+    }
+    // Sutherland-Hodgman against x <= e1, -x <= e1, y <= e2, -y <= e2
+    int cur = 0;
+    for (int pl = 0; pl < 4 && np > 0; ++pl) {
+        const int ax = pl >> 1;
+        const float sg = (pl & 1) ? -1.0f : 1.0f, lim = ax ? e2 : e1;
+        int no = 0;
+        for (int q = 0; q < np; ++q) {
+            const float* pc = poly[cur][q];
+            const float* pp = poly[cur][q == 0 ? np - 1 : q - 1];
+            const float dc = pc[ax] * sg - lim, dp = pp[ax] * sg - lim;
+            if ((dc <= 0.0f) != (dp <= 0.0f)) {
+                const float t = dp / (dp - dc);
+                for (int k = 0; k < 3; ++k) poly[1 - cur][no][k] = pp[k] + (pc[k] - pp[k]) * t;
+                ++no;
+            }
+            if (dc <= 0.0f) {
+                for (int k = 0; k < 3; ++k) poly[1 - cur][no][k] = pc[k];
+                ++no;
+            }
+        }
+        np = no;
+        cur = 1 - cur;
+    }
+    float key[AGX_CONTACT_MAX];
+    int id[AGX_CONTACT_MAX];
+    int nc = 0;
+    for (int q = 0; q < np; ++q) {
+        const float* pq = poly[cur][q];
+        if (pq[2] > co) continue;
+        ContactPt pt;
+        const float hs = pq[2] * 0.5f;
+        for (int k = 0; k < 3; ++k) {
+            pt.p[k] = fc[k] + t1[k] * pq[0] + t2[k] * pq[1] + nr[k] * hs;
+            pt.n[k] = n[k];
+        }
+        pt.depth = -pq[2];
+        nc = contact_insert(c, key, id, nc, pt, pq[2], q);
+    }
+    return nc;
+}
+
+// one contact of the env's list: the pair's bodies (i < j), and the solve's per-contact state
+struct ObstacleContact {
+    ContactPt c;   // normal from body i to body j
+    int i, j;
+    float kn, bias, ln, lt[3];
+};
+
+// Sequential impulses over the env's contact list in order, `iterations` passes: obstacle_ground_row's per-contact step with body j
+// in the place of the body and body i in the place of the ground.  Relative velocity u_j(p) - u_i(p), u = v + w x (p - x); inverse
+// effective mass along d: the sum of both bodies' 1/m + (s x d) . I_w^-1 (s x d), s = p - c; impulse +dP to j, -dP to i.  A
+// kinematic body (not free) is read and never changed.  Every body of the list needs to be loaded in B.
+AGX_DEV void obstacle_contacts_solve(const AgxContactParams& P, ContactBody* B, ObstacleContact* L, int n) {
+    for (int q = 0; q < n; ++q) {
+        ObstacleContact& o = L[q];
+        const ContactBody& bi = B[o.i];
+        const ContactBody& bj = B[o.j];
+        float si[3], sj[3];
+        for (int k = 0; k < 3; ++k) {
+            si[k] = o.c.p[k] - bi.c[k];
+            sj[k] = o.c.p[k] - bj.c[k];
+            o.lt[k] = 0.0f;
+        }
+        o.kn = ckeff(sj, o.c.n, bj.inv_m, bj.Iw) + ckeff(si, o.c.n, bi.inv_m, bi.Iw);
+        o.bias = fminf(fmaxf(o.c.depth - P.rest_offset, 0.0f) / P.dt, P.max_depenetration_velocity);
+        o.ln = 0.0f;
+    }
+    for (int it = 0; it < P.iterations; ++it) {
+        for (int q = 0; q < n; ++q) {
+            ObstacleContact& o = L[q];
+            ContactBody& bi = B[o.i];
+            ContactBody& bj = B[o.j];
+            const float* nn = o.c.n;
+            float ri[3], rj[3], si[3], sj[3];
+            for (int k = 0; k < 3; ++k) {
+                ri[k] = o.c.p[k] - bi.x[k];
+                rj[k] = o.c.p[k] - bj.x[k];
+                si[k] = o.c.p[k] - bi.c[k];
+                sj[k] = o.c.p[k] - bj.c[k];
+            }
+            float vr[3], u[3], dP[3], nP[3];
+            // normal: accumulated impulse >= 0, target separating velocity bias
+            cvel(bj.v, bj.w, rj, vr);
+            cvel(bi.v, bi.w, ri, u);
+            for (int k = 0; k < 3; ++k) vr[k] = vr[k] - u[k];
+            float dl = (o.bias - cdot(nn, vr)) / o.kn;
+            const float l1 = fmaxf(o.ln + dl, 0.0f);
+            dl = l1 - o.ln;
+            o.ln = l1;
+            for (int k = 0; k < 3; ++k) {
+                dP[k] = nn[k] * dl;
+                nP[k] = -dP[k];
+            }
+            if (bj.free) cbody_apply(dP, sj, bj);
+            if (bi.free) cbody_apply(nP, si, bi);
+            // friction: drive the tangential relative velocity at p to 0, accumulated impulse inside the circle mu * ln
+            cvel(bj.v, bj.w, rj, vr);
+            cvel(bi.v, bi.w, ri, u);
+            for (int k = 0; k < 3; ++k) vr[k] = vr[k] - u[k];
+            const float vn = cdot(nn, vr);
+            float vt[3], l2[3];
+            for (int k = 0; k < 3; ++k) {
+                vt[k] = vr[k] - nn[k] * vn;
+                l2[k] = o.lt[k];
+            }
+            const float s = sqrtf(cdot(vt, vt));
+            if (s > 0.0f) {
+                float t[3];
+                for (int k = 0; k < 3; ++k) t[k] = vt[k] / s;
+                const float dt_ = s / (ckeff(sj, t, bj.inv_m, bj.Iw) + ckeff(si, t, bi.inv_m, bi.Iw));
+                for (int k = 0; k < 3; ++k) l2[k] = l2[k] - t[k] * dt_;
+            }
+            const float mag = sqrtf(cdot(l2, l2)), lim = P.friction * o.ln;
+            if (mag > lim) {
+                const float f = lim / mag;
+                for (int k = 0; k < 3; ++k) l2[k] = l2[k] * f;
+            }
+            for (int k = 0; k < 3; ++k) {
+                dP[k] = l2[k] - o.lt[k];
+                o.lt[k] = l2[k];
+                nP[k] = -dP[k];
+            }
+            if (bj.free) cbody_apply(dP, sj, bj);
+            if (bi.free) cbody_apply(nP, si, bi);
+        }
+    }
+}
+
 }  // namespace agx

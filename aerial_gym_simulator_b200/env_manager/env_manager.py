@@ -30,7 +30,11 @@ Differences that are deliberate and documented (DESIGN.md):
       - ... and args['contact_obstacle_ground'] = True (needs create_ground_plane): the free obstacles also meet the ground plane.
         Each sub-step, right after the obstacles advance, agx_obstacle_ground_contact stops every obstacle whose geometry's vertices
         are below the plane (one-body solve against the ground, the same write-back), before the scene is re-posed and the robot
-        moves.  Obstacle-obstacle contact is not modelled.
+        moves.
+      - ... and args['contact_obstacle_obstacle'] = True: the free obstacles also collide with each other.  Every asset must be
+        exactly one <box>.  Each sub-step, after the obstacle advance and the ground solve, agx_obstacle_obstacle_contact finds the
+        box-box contacts of every env (separating axes, clipped faces, edge pairs) and resolves them between the two free bodies
+        (the same per-contact step and write-back), before the scene is re-posed and the robot moves.
 """
 from __future__ import annotations
 
@@ -47,9 +51,9 @@ from .. import _lib
 from .. import robots  # noqa: F401  (registers robots + controllers)
 from .. import urdf
 from ..hp1 import Hp1Engine
-from ..hp2 import ContactMotion, ObstacleHull, ObstacleMass, RayScene, RaySensor
+from ..hp2 import ContactMotion, ObstacleBoxes, ObstacleHull, ObstacleMass, RayScene, RaySensor
 from ..hp2 import contact as hp2_contact
-from ..hp2 import obstacle_ground_contact
+from ..hp2 import obstacle_ground_contact, obstacle_obstacle_contact
 from ..registry._core import env_config_registry, robot_registry, sim_config_registry
 
 
@@ -103,6 +107,13 @@ def _hull_vertices(parts):
     v = np.concatenate([t.reshape(-1, 3) for _, _, t, _ in parts]) if parts else np.zeros((0, 3), np.float32)
     _, first = np.unique(v, axis=0, return_index=True)
     return v[np.sort(first)]
+
+
+def _obstacle_box_row(parts, path):
+    """the ObstacleBoxes row of a free obstacle asset whose scene parts (urdf.visual_parts) are exactly one <box>"""
+    if len(parts) != 1 or parts[0][3] is None or parts[0][3][15] != 2.0:
+        raise ValueError(f"{path}: args['contact_obstacle_obstacle'] needs every obstacle asset to be exactly one <box>")
+    return ObstacleBoxes.row(parts[0][3])
 
 
 def _quat_rotate_inverse(q, v):
@@ -187,6 +198,12 @@ class EnvManager:
         if ground and not bool(getattr(self.cfg.env, "create_ground_plane", False)):
             raise ValueError("args['contact_obstacle_ground'] needs an env with create_ground_plane")
         self.contact_obstacle_ground = ground
+        pairs = self.env_args.get("contact_obstacle_obstacle", False)
+        if not isinstance(pairs, bool):
+            raise ValueError("args['contact_obstacle_obstacle'] must be a bool")
+        if pairs and not dynamic:
+            raise ValueError("args['contact_obstacle_obstacle'] needs args['contact_dynamic_obstacles'] = True")
+        self.contact_obstacle_obstacle = pairs
         self.global_tensor_dict = {}
         self.step_counter = 0
         self._graphs, self._dist_ctr_dev = {}, None
@@ -302,6 +319,11 @@ class EnvManager:
         self._obstacle_hull = None
         if self._obstacle_mass is not None and self.contact_obstacle_ground:
             self._obstacle_hull = ObstacleHull.from_files(self._hull_files, self._asset_file, dev)
+        # the obstacle-obstacle solve: every asset's box (table built in _build_obstacles)
+        self._obstacle_boxes = None
+        if self._obstacle_mass is not None and self.contact_obstacle_obstacle:
+            self._obstacle_boxes = ObstacleBoxes(torch.from_numpy(np.stack(self._box_rows)).to(dev),
+                                                 torch.from_numpy(self._asset_box).to(dev))
 
     # ---- obstacles: AssetLoader.select_assets_for_sim + WarpEnv (asset_loader.py:148-194, warp_env_manager.py)
     def _select_assets(self):
@@ -372,6 +394,9 @@ class EnvManager:
         # obstacle-ground contact: the vertices of each distinct URDF's scene parts, and each asset's file
         ground = self.contact_obstacle_ground
         file_of, hull_files, asset_file = {}, [], (np.zeros((N, A), np.int32) if ground else None)
+        # obstacle-obstacle contact: the box of each distinct URDF, and each asset's box
+        pairs = self.contact_obstacle_obstacle
+        box_of, box_rows, asset_box = {}, [], (np.zeros((N, A), np.int32) if pairs else None)
         for e in range(N):
             for a, (params, path) in enumerate(per_env[e]):
                 lo[e, a], hi[e, a] = params.min_state_ratio, params.max_state_ratio
@@ -387,6 +412,9 @@ class EnvManager:
                     if ground:
                         file_of[path] = len(hull_files)
                         hull_files.append(_hull_vertices(parts))
+                    if pairs:
+                        box_of[path] = len(box_rows)
+                        box_rows.append(_obstacle_box_row(parts, path))
                     for _, link_index, tris, obb in parts:
                         if obb is None:
                             ids.append(-1 - len(meshes))
@@ -402,10 +430,14 @@ class EnvManager:
                     asset_mass[e, a] = mass_of[path]
                 if ground:
                     asset_file[e, a] = file_of[path]
+                if pairs:
+                    asset_box[e, a] = box_of[path]
         if dynamic:
             self._asset_mass = torch.from_numpy(asset_mass)
         if ground:
             self._hull_files, self._asset_file = hull_files, asset_file
+        if pairs:
+            self._box_rows, self._asset_box = box_rows, asset_box
         gtd["asset_min_state_ratio"].copy_(torch.from_numpy(lo))
         gtd["asset_max_state_ratio"].copy_(torch.from_numpy(hi))
         if not self.use_warp:
@@ -691,7 +723,8 @@ class EnvManager:
         Dynamic obstacles (args['contact_dynamic_obstacles'], fixed for the manager, so (n, moving) keys the graph): every sub-step
         advances the obstacles, with the env_actions twist when moving and with their own velocity otherwise, the solve writes the
         obstacles it pushes, and the scene is re-posed once more after the last sub-step.  With args['contact_obstacle_ground'] (also
-        fixed for the manager) each sub-step's obstacle advance is followed by the obstacle-ground solve."""
+        fixed for the manager) each sub-step's obstacle advance is followed by the obstacle-ground solve, and with
+        args['contact_obstacle_obstacle'] (fixed too) by the obstacle-obstacle solve after it."""
         g = self._graphs.get((n, moving))
         if g is not None:
             return g
@@ -843,12 +876,14 @@ class EnvManager:
 
     def _move_obstacles_one_substep(self, with_twist=True):
         """contact with moving obstacles: one sub-step of the obstacles (the advance keeps its state in float32, so n of these add
-        up bit for bit to one n-sub-step advance), with args['contact_obstacle_ground'] the obstacle-ground solve, and the scene
-        re-posed where they now are.  with_twist False (dynamic obstacles in a step without env_actions): each obstacle keeps its own
+        up bit for bit to one n-sub-step advance), with args['contact_obstacle_ground'] the obstacle-ground solve, with
+        args['contact_obstacle_obstacle'] the obstacle-obstacle solve, and the scene re-posed where they now are.  with_twist False (dynamic obstacles in a step without env_actions): each obstacle keeps its own
         damped velocity."""
         self._advance_obstacles(self.global_tensor_dict["env_actions"] if with_twist else None, 1)
         if self._obstacle_hull is not None:  # obstacle-ground contact: the robot's contact search sees the corrected obstacles
             obstacle_ground_contact(self.contact_params, self._contact_motion, self._obstacle_mass, self._obstacle_hull)
+        if self._obstacle_boxes is not None:  # obstacle-obstacle contact: after the ground's, so the scene shows both corrections
+            obstacle_obstacle_contact(self.contact_params, self._contact_motion, self._obstacle_mass, self._obstacle_boxes)
         self._repose_scene()
 
     def compute_observations(self, moving_obstacles=False):

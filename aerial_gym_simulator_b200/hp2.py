@@ -370,6 +370,73 @@ class ObstacleHull:
         return cls(*(torch.from_numpy(np.ascontiguousarray(x)).to(device) for x in (v, off, reach, np.asarray(asset_file))))
 
 
+class ObstacleBoxes:
+    """The box table of the obstacle–obstacle contact (agx_obstacle_obstacle_contact), one AgxObstacleBoxes.
+    boxes: float32 [F,15], each file's box in the asset frame: centre (3), the three unit axes (3 each; box_obb's layout), the half
+    extents (3); asset_file: integer [E,A], the file of each (env, asset).  Checked here once (one host read): finite values, half
+    extents >= 0, axes orthonormal to 1e-5, every asset_file in [0, F).  Kept as contiguous copies on boxes' device (int32 indices)."""
+
+    def __init__(self, boxes: torch.Tensor, asset_file: torch.Tensor):
+        for name, x, fp in (("boxes", boxes, True), ("asset_file", asset_file, False)):
+            if not isinstance(x, torch.Tensor) or x.is_floating_point() != fp or x.dtype == torch.bool or x.is_complex():
+                raise ValueError(f"{name} must be a{' floating-point' if fp else 'n integer'} tensor")
+        dev = boxes.device
+        b = boxes.to(device=dev, dtype=torch.float32).contiguous()
+        af = asset_file.to(device=dev, dtype=torch.int32).contiguous()
+        if b.dim() != 2 or b.shape[0] < 1 or b.shape[1] != 15:
+            raise ValueError("boxes must be [F>=1,15]")
+        if af.dim() != 2 or af.shape[1] < 1:
+            raise ValueError("asset_file must be [E,A>=1]")
+        F = b.shape[0]
+        ax = b[:, 3:12].double().view(F, 3, 3)
+        gram = ax @ ax.transpose(1, 2)
+        checks = torch.stack([torch.isfinite(b).all(), (b[:, 12:15] >= 0).all(),
+                              ((gram - torch.eye(3, dtype=gram.dtype, device=dev)).abs() <= 1e-5).all(),
+                              (af >= 0).all(), (af < F).all()]).cpu()
+        msgs = ("boxes must be finite", "box half extents must be >= 0", "box axes must be orthonormal",
+                f"asset_file values must be in [0, {F})", f"asset_file values must be in [0, {F})")
+        for ok, msg in zip(checks.tolist(), msgs):
+            if not ok:
+                raise ValueError(msg)
+        self.boxes, self.asset_file = b, af
+        self.E, self.A, self.F, self.device = af.shape[0], af.shape[1], F, dev
+        self.c = _lib.AgxObstacleBoxes(boxes=b.data_ptr(), asset_file=af.data_ptr(), num_files=F)
+
+    @staticmethod
+    def row(obb) -> np.ndarray:
+        """the [15] table row of a box from its box_obb record (centre, axes, half extents; the kind is dropped)"""
+        return np.asarray(obb, np.float32)[0:15].copy()
+
+
+def obstacle_obstacle_contact(params: _lib.AgxContactParams, motion: ContactMotion, mass: ObstacleMass, boxes: ObstacleBoxes):
+    """agx_obstacle_obstacle_contact: the free obstacle assets of motion.asset_state [E,A,>=13] against each other, one oriented box
+    each (boxes); the rows with a contact get their new twist and position correction in place.  A <= 64.  Of params only
+    contact_offset, rest_offset, dt, friction, max_depenetration_velocity and iterations are read."""
+    if not isinstance(params, _lib.AgxContactParams):
+        raise ValueError("params must be an AgxContactParams")
+    if not isinstance(motion, ContactMotion):
+        raise ValueError("motion must be a ContactMotion")
+    if not isinstance(mass, ObstacleMass):
+        raise ValueError("mass must be an ObstacleMass")
+    if not isinstance(boxes, ObstacleBoxes):
+        raise ValueError("boxes must be an ObstacleBoxes")
+    st = motion.asset_state
+    dev = st.device
+    E, A = st.shape[0], st.shape[1]
+    if (mass.E, mass.A) != (E, A) or mass.device != dev:
+        raise ValueError("mass must have one row per motion asset [E,A], on the asset rows' device")
+    if (boxes.E, boxes.A) != (E, A) or boxes.device != dev:
+        raise ValueError("boxes must have one file index per motion asset [E,A], on the asset rows' device")
+    if A > _lib.OBSTACLE_MAX_ASSETS:
+        raise ValueError(f"obstacle_obstacle_contact takes at most {_lib.OBSTACLE_MAX_ASSETS} assets per env, not {A}")
+    if dev.type != "cuda":
+        raise _lib.AgxError("obstacle_obstacle_contact needs a CUDA device: there is no CPU path")
+    _lib.check(_lib.load().agx_obstacle_obstacle_contact(E, A, C.byref(params), C.c_void_p(st.data_ptr()), st.stride(1),
+                                                         C.c_void_p(mass.table.data_ptr()), C.byref(boxes.c),
+                                                         C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)),
+               "agx_obstacle_obstacle_contact")
+
+
 def obstacle_ground_contact(params: _lib.AgxContactParams, motion: ContactMotion, mass: ObstacleMass, hull: ObstacleHull):
     """agx_obstacle_ground_contact: every free obstacle asset of motion.asset_state [E,A,>=13] against the ground plane z = 0 through
     the vertices of its file in hull; the rows with a kept contact get their new twist and position correction in place.  Of params

@@ -173,7 +173,8 @@ const char* agx_last_error(void);
 /* sizeof() of the ABI structs as compiled into the library (binding self-check):
  * which = 0 AgxHp1Config, 1 AgxHp1Buffers, 2 AgxHp1ResetDraws, 3 AgxHp2Scene, 4 AgxHp2Sensor,
  * 5 AgxNavRewardParams, 6 AgxImuConfig, 7 AgxLidarNavRewardParams, 8 AgxHp2Noise, 9 AgxE2ERewardParams, 10 AgxObsGatherPush,
- * 11 AgxContactParams, 12 AgxContactMotion, 13 AgxObstacleMass, 14 AgxObstacleHull, 15 AgxArticulation */
+ * 11 AgxContactParams, 12 AgxContactMotion, 13 AgxObstacleMass, 14 AgxObstacleHull, 15 AgxArticulation,
+ * 16 AgxObstacleBoxes */
 uint64_t agx_sizeof(int which);
 
 /* Host buffers the kernels can address directly (pinned, portable, mapped: cudaHostAlloc).
@@ -667,6 +668,32 @@ typedef struct AgxObstacleHull {
  * (radius, mass, inertia_inv, com, force_threshold, ground_plane) are ignored.  mass [E,A] as agx_hp2_contact_dynamic's. */
 int agx_obstacle_ground_contact(int num_envs, int num_assets, const AgxContactParams* params, float* asset_state, int asset_stride,
                                 const AgxObstacleMass* mass, const AgxObstacleHull* hull, void* stream);
+
+/* Contact between free obstacles (DESIGN.md "Contact mode", "Contact between free obstacles"): every free obstacle asset is one
+ * oriented box.  boxes[f*15 ..] is file f's box in the asset frame: centre (3), the three unit axes (3 each), the half extents (3);
+ * asset a of env e uses file asset_file[e,a].  Every value of asset_file is in [0, num_files): the caller checks this when it builds
+ * the table, the kernel reads without a bounds check. */
+typedef struct AgxObstacleBoxes {
+    const float* boxes;         /* [F,15] */
+    const int32_t* asset_file;  /* [E,A] */
+    int32_t num_files;          /* F >= 1 */
+} AgxObstacleBoxes;
+
+#define AGX_OBSTACLE_MAX_ASSETS 64     /* num_assets limit of agx_obstacle_obstacle_contact (the env's bodies live in shared memory) */
+#define AGX_OBSTACLE_MAX_CONTACTS 128  /* contact-list capacity per env */
+
+/* One warp per env of asset_state [E,A,asset_stride] (rows as agx_obstacle_ground_contact's, read AND written), A <= 64.
+ * Broad phase: every pair (i < j) whose bounding spheres (centre, radius |half extents|) are within contact_offset, unless both are
+ * kinematic.  Narrow phase: the separating-axis test on the 15 box-box axes within contact_offset, the minimum-penetration axis
+ * (B's face over A's, an edge pair over the faces, only when better by more than 1e-4 m) and up to AGX_CONTACT_MAX contacts: the
+ * incident face clipped against the reference face, or the closest points of two edges (contact_core.cuh obstacle_box_pair).
+ * The env's contact list is every kept contact in (i, j, contact index) order; a pair whose contacts no longer fit in
+ * AGX_OBSTACLE_MAX_CONTACTS is dropped with every later pair.  Solve: agx_obstacle_ground_contact's per-contact step with body j in
+ * place of the body and body i in place of the ground (relative velocity u_j(p) - u_i(p), both bodies' inverse effective masses,
+ * +dP to j, -dP to i), over the whole list, `iterations` passes; then every free body with a contact gets the same write-back.
+ * Kinematic rows (all-zero mass entry) are read and never written.  Params and mass as agx_obstacle_ground_contact's. */
+int agx_obstacle_obstacle_contact(int num_envs, int num_assets, const AgxContactParams* params, float* asset_state, int asset_stride,
+                                  const AgxObstacleMass* mass, const AgxObstacleBoxes* boxes, void* stream);
 
 
 /* ======================================================================================
