@@ -213,6 +213,8 @@ def load():
         "agx_hp1_position_task_step_profiled": [C.POINTER(AgxHp1Config), C.POINTER(AgxHp1Buffers), C.c_void_p,
                                                 C.c_void_p],
         "agx_hp1_articulated_step": [C.POINTER(AgxHp1Config), C.POINTER(AgxHp1Buffers), C.POINTER(AgxArticulation), C.c_void_p],
+        "agx_hp1_articulated_step_imu": [C.POINTER(AgxHp1Config), C.POINTER(AgxHp1Buffers), C.POINTER(AgxArticulation), C.c_int,
+                                         C.c_void_p, C.c_void_p],
         "agx_hp1_articulated_body_state": [C.POINTER(AgxArticulation), C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p],
         "agx_hp1_reset": [C.POINTER(AgxHp1Config), C.POINTER(AgxHp1Buffers), C.c_void_p,
                           C.POINTER(AgxHp1ResetDraws), C.c_void_p],

@@ -4,8 +4,9 @@ Articulated robots (ROV, reconfigurable, Morphy) are out of the hot-path scope (
 import numpy as np
 
 from . import RESOURCES_DIRECTORY
-from .sensor_config import (BaseDepthCameraConfig, BaseImuConfig, BaseLidarConfig, BaseNormalFaceIDCameraConfig, GimbalDepthCameraConfig,
-                            OSDome_64_Config, RSLidar_Airy_Config, StereoCameraConfig, fake_radar_config, pmd_flexx2_config)
+from .sensor_config import (BaseDepthCameraConfig, BaseImuConfig, BaseLidarConfig, BaseLinkImuConfig, BaseNormalFaceIDCameraConfig,
+                            GimbalCameraImuConfig, GimbalDepthCameraConfig, OSDome_64_Config, RSLidar_Airy_Config, StereoCameraConfig,
+                            fake_radar_config, pmd_flexx2_config)
 
 PI = np.pi
 QUAD_ALLOCATION = [
@@ -499,3 +500,21 @@ class BaseQuadWithGimbalCameraCfg(BaseQuadCfg):
         max_init_dof_position = 0.0
         min_init_dof_velocity = 0.0
         max_init_dof_velocity = 0.0
+
+
+class BaseQuadWithGimbalCameraImuCfg(BaseQuadWithGimbalCameraCfg):
+    """base_quadrotor_with_gimbal_camera with an IMU on gimbal_camera_link (GimbalCameraImuConfig): imu_measurement is the levelled
+    camera's specific force and angular rate"""
+    class sensor_config(BaseQuadWithGimbalCameraCfg.sensor_config):
+        enable_imu = True
+        imu_config = GimbalCameraImuConfig
+
+    class robot_asset(BaseQuadWithGimbalCameraCfg.robot_asset):
+        name = "base_quadrotor_with_gimbal_camera_imu"
+
+
+class MorphyCompliantImuCfg(MorphyCompliantCfg):
+    """morphy_compliant with an IMU on base_link: its force input includes the arms' joint reactions"""
+    class sensor_config(MorphyCompliantCfg.sensor_config):
+        enable_imu = True
+        imu_config = BaseLinkImuConfig

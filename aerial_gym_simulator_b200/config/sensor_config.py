@@ -206,6 +206,19 @@ class BaseImuConfig(BaseSensorConfig):
     max_euler_rotation_deg = [2.0, 2.0, 2.0]
 
 
+class BaseLinkImuConfig(BaseImuConfig):
+    """an IMU on base_link (ours): on an articulated robot an IMU names its link; its force input is the base body's, the arms'
+    joint reactions included"""
+    parent_link = "base_link"
+
+
+class GimbalCameraImuConfig(BaseImuConfig):
+    """an IMU on gimbal_camera_link of quad_gimbal.urdf (ours), next to the gimbal's camera: parent_link makes EnvManager read the
+    force, orientation and angular velocity of that link's body (the gimbal's pitch stage), so the IMU measures what the levelled
+    camera feels, as a gimbal controller's own IMU does"""
+    parent_link = "gimbal_camera_link"
+
+
 class BoschBMI088Config(BaseImuConfig):
     """imu_config/bosch_bmi088_config.py"""
     bias_std = [0.0013564659966250536] * 3 + [1.4352700094407325e-05] * 3

@@ -63,6 +63,22 @@ ArtKernel pick_art_kernel(int M, int B) {
     return B <= 9 ? articulated_step_kernel<8, 9> : articulated_step_kernel<8, AGX_ART_MAX_BODIES>;
 }
 
+// ---- the step with the IMU input of one body (agx_hp1_articulated_step_imu): articulated_step_kernel plus one [9] store per env
+template <int M, int NB>
+__global__ void __launch_bounds__(kArtThreads)
+articulated_step_imu_kernel(const __grid_constant__ AgxHp1Config cfg, const __grid_constant__ AgxHp1Buffers buf,
+                            const __grid_constant__ AgxArticulation art, int imu_body, float* __restrict__ imu_input) {
+    const int env = blockIdx.x * blockDim.x + threadIdx.x;
+    if (env >= cfg.num_envs) return;
+    art_env_step<M, NB, true>(cfg, buf, art, env, imu_body, imu_input);
+}
+
+using ArtImuKernel = void (*)(const AgxHp1Config, const AgxHp1Buffers, const AgxArticulation, int, float*);
+ArtImuKernel pick_art_imu_kernel(int M, int B) {
+    if (M == 4) return B <= 9 ? articulated_step_imu_kernel<4, 9> : articulated_step_imu_kernel<4, AGX_ART_MAX_BODIES>;
+    return B <= 9 ? articulated_step_imu_kernel<8, 9> : articulated_step_imu_kernel<8, AGX_ART_MAX_BODIES>;
+}
+
 // ---- per-body state (agx_hp1_articulated_body_state) ----------------------------------------------------------------------
 // One env per lane, one warp per block.  Each lane builds its env's B rows (13 B floats) in shared memory with art_body_states, the
 // rows of the parents serving as the sweep's scratch, so nothing goes to local memory.  Written straight from the lanes, the rows
@@ -144,4 +160,18 @@ extern "C" int agx_hp1_articulated_step(const AgxHp1Config* cfg, const AgxHp1Buf
     const int g = (cfg->num_envs + kArtThreads - 1) / kArtThreads;
     pick_art_kernel(cfg->num_motors, art->num_bodies)<<<g, kArtThreads, 0, (cudaStream_t)stream>>>(*cfg, *buf, *art);
     return agx_check_launch("articulated_step_kernel");
+}
+
+extern "C" int agx_hp1_articulated_step_imu(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, const AgxArticulation* art, int imu_body,
+                                            float* imu_input, void* stream) {
+    int rc = validate_articulation(cfg, buf, art);
+    if (rc) return rc;
+    if (imu_body < 0 || imu_body >= art->num_bodies)
+        return agx_set_error(AGX_E_INVALID, "imu_body must be in [0, %d) (got %d)", art->num_bodies, imu_body);
+    if (!imu_input) return agx_set_error(AGX_E_NULL, "imu_input is NULL");
+    if (cfg->num_envs == 0) return AGX_OK;
+    const int g = (cfg->num_envs + kArtThreads - 1) / kArtThreads;
+    pick_art_imu_kernel(cfg->num_motors, art->num_bodies)<<<g, kArtThreads, 0, (cudaStream_t)stream>>>(*cfg, *buf, *art, imu_body,
+                                                                                                      imu_input);
+    return agx_check_launch("articulated_step_imu_kernel");
 }

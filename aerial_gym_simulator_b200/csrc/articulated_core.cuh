@@ -120,6 +120,50 @@ AGX_DEV void spd6_solve(const float* A, const float* b, float* x) {
     }
 }
 
+// R^T v
+AGX_DEV V3 mul33tv(const M33& A, V3 v) {
+    return V3{A.m[0] * v.x + A.m[3] * v.y + A.m[6] * v.z, A.m[1] * v.x + A.m[4] * v.y + A.m[7] * v.z,
+              A.m[2] * v.x + A.m[5] * v.y + A.m[8] * v.z};
+}
+
+// ---- the IMU input of one body (agx_hp1_articulated_step_imu) ---------------------------------------------------------------
+// From what the ABA holds for body b at the sub-step's start: its rotation R and origin P (relative to O), its spatial velocity
+// V = (w, v_O) and acceleration A = (alpha, a^), both in world axes about O.  COM c = P + R com_b, its classical acceleration
+// a_c = a^ + alpha x c + w x (v_O + w x c).  out [9] = (f, n, w_b), all in body b's frame:
+//   f = m_b R^T (a_c - g)                       the non-gravitational force on the body, joint reactions included
+//   n = I_b R^T alpha + w_b x I_b w_b            the net torque about the COM (I_b about the COM, body axes)
+//   w_b = R^T w
+AGX_DEV void art_imu_input(const AgxArticulation& art, int b, const M33& R, V3 P, const float* V, const float* A, V3 grav, float* out) {
+    const V3 w = sv_ang(V), al = sv_ang(A);
+    const V3 c = P + mul33v(R, ld3(art.com[b]));
+    const V3 ac = sv_lin(A) + cross(al, c) + cross(w, sv_lin(V) + cross(w, c));
+    const V3 f = mul33tv(R, (ac - grav) * art.mass[b]);
+    const V3 wb = mul33tv(R, w), ab = mul33tv(R, al);
+    const M33 Ib = ld33(art.inertia[b]);
+    const V3 n = mul33v(Ib, ab) + cross(wb, mul33v(Ib, wb));
+    out[0] = f.x; out[1] = f.y; out[2] = f.z;
+    out[3] = n.x; out[4] = n.y; out[5] = n.z;
+    out[6] = wb.x; out[7] = wb.y; out[8] = wb.z;
+}
+
+// w_b = R_b^T w_b of body b without the dynamics (the IMU input of a launch with physics_steps = 0): the forward kinematics of
+// art_dynamics along the bodies 0..b
+template <int NB>
+AGX_DEV V3 art_body_angvel(const AgxArticulation& art, const EnvState& s, const float* q, const float* qd, int b) {
+    M33 R[NB];
+    V3 W[NB];
+    R[0] = quat_to_matrix(s.q);
+    W[0] = s.w;
+    for (int i = 1; i <= b; ++i) {
+        const int l = art.parent[i];
+        const V3 ax = ld3(art.axis[i]);
+        const M33 RJ = mul33(R[l], ld33(art.joint_R[i]));
+        R[i] = mul33(RJ, axis_angle(ax, q[i - 1]));
+        W[i] = W[l] + mul33v(RJ, ax) * qd[i - 1];
+    }
+    return mul33tv(R[b], W[b]);
+}
+
 // ---- the dynamics of one sub-step ------------------------------------------------------------------------------------------
 // In: base pose / twist s (root-origin velocity v, world angular velocity w), joint q, qd and drive targets qs, qds, motor thrusts
 // (M motors), the base's external force F_w / torque T_w (world frame, force acting at the base origin), gravity, dt.
@@ -127,9 +171,11 @@ AGX_DEV void spd6_solve(const float* A, const float* b, float* x) {
 // origin: that is a0_lin + w x v), qdd[D].
 // The joint drive tau = k (qs - q') + d (qds - qd') is taken at the end-of-step q' = q + dt qd', qd' = qd + dt qdd: its implicit part
 // moves into the joint's pivot D_i = S^T I^A S + dt d + dt^2 k, the explicit part k (qs - q - dt qd) + d (qds - qd) into u_i.
-template <int NB>
+// IMU: where imu != NULL, also art_imu_input of body imu_body into imu[9]; a0 and qdd are the same either way.
+template <int NB, bool IMU = false>
 AGX_DEV void art_dynamics(const AgxArticulation& art, const EnvState& s, const float* q, const float* qd, const float* qs,
-                          const float* qds, float dt, V3 grav, int M, const float* thrust, V3 F_w, V3 T_w, float* a0, float* qdd) {
+                          const float* qds, float dt, V3 grav, int M, const float* thrust, V3 F_w, V3 T_w, float* a0, float* qdd,
+                          int imu_body = 0, float* imu = nullptr) {
     const int B = art.num_bodies;
     M33 R[NB];
     V3 P[NB];
@@ -230,6 +276,9 @@ AGX_DEV void art_dynamics(const AgxArticulation& art, const EnvState& s, const f
 #pragma unroll
         for (int r = 0; r < 6; ++r) A[i][r] = ai[r] + S[i][r] * x;
     }
+    if constexpr (IMU) {
+        if (imu) art_imu_input(art, imu_body, R[imu_body], P[imu_body], V[imu_body], A[imu_body], grav, imu);
+    }
 }
 
 // ---- integration: the base by the HP1 integrator spec (DESIGN.md section 3, integrate() of hp1_core.cuh) on the accelerations
@@ -294,8 +343,11 @@ AGX_DEV void art_load_params(const AgxHp1Config& cfg, const AgxHp1Buffers& buf, 
 // Each sub-step: update_states -> controller -> allocation -> motor model (hp1_core.cuh), drag on the base (body-frame velocities
 // of the base origin, base_multirotor.py:260-285) plus the disturbance, then the articulated dynamics and the integration.
 // Derived states d are those of the last sub-step's start (agx_hp1_physics_step's staleness).
-template <int M, int NB>
-AGX_DEV void art_env_step(const AgxHp1Config& cfg, const AgxHp1Buffers& buf, const AgxArticulation& art, int env) {
+// IMU: also the IMU input of body imu_body into imu_input [N,9] -- art_imu_input on the last sub-step; with physics_steps = 0,
+// f = n = 0 and w_b of the unstepped state (agx_hp1_physics_step's body_wrench is zero then).  The state arithmetic is unchanged.
+template <int M, int NB, bool IMU = false>
+AGX_DEV void art_env_step(const AgxHp1Config& cfg, const AgxHp1Buffers& buf, const AgxArticulation& art, int env, int imu_body = 0,
+                          float* imu_input = nullptr) {
     EnvParams<M> p;
     art_load_params<M>(cfg, buf, env, p);
     const int A = cfg.num_actions;
@@ -350,10 +402,24 @@ AGX_DEV void art_env_step(const AgxHp1Config& cfg, const AgxHp1Buffers& buf, con
             dtq = dtq + V3{d6[3], d6[4], d6[5]};
         }
         float a0[6];
-        art_dynamics<NB>(art, s, q, qd, qs, qds, cfg.dt, grav, M, p.thrust, quat_rotate(s.q, df), quat_rotate(s.q, dtq), a0, qdd);
+        if constexpr (IMU) {
+            float* imu = (step + 1 == cfg.physics_steps) ? imu_input + (size_t)env * 9 : nullptr;
+            art_dynamics<NB, true>(art, s, q, qd, qs, qds, cfg.dt, grav, M, p.thrust, quat_rotate(s.q, df), quat_rotate(s.q, dtq), a0,
+                                   qdd, imu_body, imu);
+        } else {
+            art_dynamics<NB>(art, s, q, qd, qs, qds, cfg.dt, grav, M, p.thrust, quat_rotate(s.q, df), quat_rotate(s.q, dtq), a0, qdd);
+        }
         art_integrate(cfg, art, s, a0, q, qd, qdd);
     }
     if (cfg.physics_steps == 0) d = update_states(s);
+    if constexpr (IMU) {
+        if (cfg.physics_steps == 0) {
+            const V3 wb = art_body_angvel<NB>(art, s, q, qd, imu_body);
+            float* o = imu_input + (size_t)env * 9;
+            o[0] = 0.0f; o[1] = 0.0f; o[2] = 0.0f; o[3] = 0.0f; o[4] = 0.0f; o[5] = 0.0f;
+            o[6] = wb.x; o[7] = wb.y; o[8] = wb.z;
+        }
+    }
     float r[13];
     pack(s, r);
 #pragma unroll

@@ -231,22 +231,33 @@ class EnvManager:
         self.spec = spec
         self.articulated = bool(getattr(self.robot, "articulated", False))
         articulation = None
+        imu_on = bool(getattr(self.robot_cfg.sensor_config, "enable_imu", False))
+        imu_link = getattr(self.robot_cfg.sensor_config.imu_config, "parent_link", None) if imu_on else None
+        # an IMU on a link (imu_config.parent_link): (link name, body, R_l = the link's frame in the body's frame)
+        self._imu_link = (imu_link, *self._resolve_link(imu_link)[:2]) if imu_link is not None else None
         if self.articulated:
             if self.contact_mode == "rigid":
                 raise ValueError("args['contact'] = 'rigid' is not available for an articulated robot: the contact solve gives its impulse "
                                  "to the base alone, which is wrong for a tree of bodies")
-            if getattr(self.robot_cfg.sensor_config, "enable_imu", False):
-                raise ValueError("the IMU is not available on an articulated robot: its force input would need the joint reaction forces")
+            if imu_on and imu_link is None:
+                raise ValueError("the IMU of an articulated robot reads the force on one body, the joint reaction forces included: "
+                                 "name the link with imu_config.parent_link")
+            if imu_on and not self.robot.bodies.mass[self._imu_link[1]] > 0:
+                raise ValueError(f"imu_config.parent_link '{imu_link}' belongs to a body without mass: the IMU divides its force by the "
+                                 "body's mass")
             if bool(self.env_args.get("host_io", False)):
                 raise NotImplementedError("args['host_io'] is a feature of the fused task step, which articulated robots do not have")
             articulation = self.robot.make_articulation()
+        extra = {"articulation": articulation} if articulation is not None else {}
+        if articulation is not None and imu_on:
+            extra["imu_body"] = self._imu_link[1]  # the step also writes that body's force input (Hp1Engine.imu_input)
         self.engine = Hp1Engine(
             spec, N, dev, physics_steps=1, seed=int(self.env_args.get("seed", 0)),
             env_id_offset=int(self.env_args.get("env_id_offset", 0)), device_rng_reset=(self.reset_rng == "device"),
             strict_stale_obs=bool(self.env_args.get("strict_stale_obs", True)), materialize_derived=True,
             per_env_params=self.env_args.get("per_env_params", "auto"), host_io=bool(self.env_args.get("host_io", False)),
-            debug_wrench=bool(getattr(self.robot_cfg.sensor_config, "enable_imu", False)),  # the IMU reads the net body force
-            **({"articulation": articulation} if articulation is not None else {}))
+            debug_wrench=imu_on and not self.articulated,  # a rigid robot's IMU reads the net body force
+            **extra)
         eng, gtd = self.engine, self.global_tensor_dict
         if articulation is not None:
             # joint state (position, velocity) and the drive targets; the targets belong to the user: the env never writes them
@@ -499,6 +510,16 @@ class EnvManager:
             gtd["force_sensor_tensor"] = torch.zeros(N, 6, device=dev)
             self.imu = IMUSensor(sc.imu_config, N, dev)
             self.imu.init_tensors(gtd)
+            if self._imu_link is not None:
+                # an IMU on a link: sensor_quats stays relative to the link, the kernel reads q_l (x) sensor_quats
+                _, b, R_l = self._imu_link
+                self.imu.set_link(torch.tensor(_matrix_to_quat(np.asarray(R_l, np.float64)), dtype=torch.float32))
+                if self.articulated:
+                    # ... and body b's force input (Hp1Engine.imu_input), mass, orientation row and angular velocity
+                    self._imu_mass = torch.full((N,), float(self.robot.bodies.mass[b]), device=dev)
+                    self._imu_angvel = torch.zeros(N, 3, device=dev)
+                    self.imu.robot_masses, self.imu.robot_state = self._imu_mass, self._body_state[:, b, :]
+                    self.imu.robot_body_angvel = self._imu_angvel
         if not self.use_warp:
             return
         if sc.enable_camera and sc.enable_lidar:
@@ -911,7 +932,16 @@ class EnvManager:
             self.render_sensors()
 
     def render_sensors(self):
-        if self.imu is not None:
+        if self.imu is not None and self.articulated:
+            # body b's force input of the last sub-step + m_b R_b^T g, R_b from its row of robot_body_state_tensor: the rigid path's
+            # line below, per body
+            fs, u = self.global_tensor_dict["force_sensor_tensor"], self.engine.imu_input
+            fs[:, 0:3] = u[:, 0:3] + self._imu_mass.unsqueeze(1) * _quat_rotate_inverse(self.imu.robot_state[:, 3:7],
+                                                                                          self.global_tensor_dict["gravity"])
+            fs[:, 3:6] = u[:, 3:6]
+            self._imu_angvel.copy_(u[:, 6:9])
+            self.imu.update()
+        elif self.imu is not None:
             gtd = self.global_tensor_dict
             fs, w = gtd["force_sensor_tensor"], self.engine.body_wrench
             fs[:, 0:3] = w[:, 0:3] + gtd["robot_mass"].unsqueeze(1) * _quat_rotate_inverse(gtd["robot_orientation"], gtd["gravity"])

@@ -273,7 +273,8 @@ class Hp1Engine:
 
     def __init__(self, spec: MultirotorSpec, num_envs: int, device="cuda:0", *, physics_steps=1,
                  episode_len_steps=500, seed=0, env_id_offset=0, device_rng_reset=True, strict_stale_obs=True,
-                 materialize_derived=True, per_env_params="auto", debug_wrench=False, host_io=False, articulation=None):
+                 materialize_derived=True, per_env_params="auto", debug_wrench=False, host_io=False, articulation=None,
+                 imu_body=None):
         """host_io: obs / reward / terminations / truncations live in pinned, device-mapped HOST
         memory (agx_host_alloc) and the fused task step stores them there directly over PCIe;
         `actions` may then be a pinned host tensor (e.g. `self.host_actions`) that the kernel
@@ -281,7 +282,10 @@ class Hp1Engine:
         articulation: an ArticulationSpec -- the robot has joints; physics_step runs agx_hp1_articulated_step and the engine owns
         dof_state [N,D,2] and the drive targets dof_position_setpoint / dof_velocity_setpoint [N,D] (zero until the caller writes
         them), and body_state [N,B,13], every body's pose and velocity, which update_body_state() refreshes.  There is no fused task
-        step for such a robot."""
+        step for such a robot.
+        imu_body: with an articulation, the body an IMU rides on -- physics_step then runs agx_hp1_articulated_step_imu, which also
+        writes imu_input [N,9] = (force f_b, torque n_b, angular velocity w_b) of that body in its own frame, of the last
+        sub-step's start (the IMU's force input; the state update is the same arithmetic)."""
         self.lib = _lib.load()
         self.device = torch.device(device)
         if self.device.type != "cuda":
@@ -293,6 +297,7 @@ class Hp1Engine:
                                 strict_stale_obs=strict_stale_obs)
         N, M, dev = self.N, self.M, self.device
         self._init_body_state()
+        self._init_imu(imu_body)
         z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=dev)
         self.root_state = z(N, 13)
         self.root_state[:, 6] = 1.0
@@ -377,6 +382,17 @@ class Hp1Engine:
         if self.articulation is not None:
             B = self.articulation.bodies.num_bodies
             self.body_state = torch.zeros(self.N, B, 13, dtype=torch.float32, device=self.device)
+
+    def _init_imu(self, imu_body):
+        """imu_input [N,9] of an articulated robot with an IMU on body imu_body (None otherwise), zero until the first step"""
+        self.imu_body, self.imu_input = None, None
+        if imu_body is None:
+            return
+        if self.articulation is None:
+            raise ValueError("imu_body belongs to an articulated robot (Hp1Engine(articulation=...)): a rigid robot's IMU reads "
+                             "body_wrench (debug_wrench=True)")
+        self.imu_body = int(imu_body)
+        self.imu_input = torch.zeros(self.N, 9, dtype=torch.float32, device=self.device)
 
     def _host_tensor(self, shape, dtype):
         nbytes = max(1, int(np.prod(shape))) * torch.empty((), dtype=dtype).element_size()
@@ -508,6 +524,10 @@ class Hp1Engine:
         self._buf.dist_offset = dist_offset
         if physics_steps is not None:
             self.cfg.physics_steps = int(physics_steps)
+        if self.imu_input is not None:
+            _lib.check(self.lib.agx_hp1_articulated_step_imu(self._cfg_ref, self._buf_ref, self._art_ref, self.imu_body,
+                                                             self.imu_input.data_ptr(), self._stream()), "agx_hp1_articulated_step_imu")
+            return
         if self.art is not None:
             _lib.check(self.lib.agx_hp1_articulated_step(self._cfg_ref, self._buf_ref, self._art_ref, self._stream()),
                        "agx_hp1_articulated_step")

@@ -148,6 +148,8 @@ for _name, _cfg in (
 robot_registry.register("base_rov", BaseROV, rc.BaseROVCfg)
 robot_registry.register("morphy_compliant", ArticulatedMultirotor, rc.MorphyCompliantCfg)
 robot_registry.register("base_quadrotor_with_gimbal_camera", ArticulatedMultirotor, rc.BaseQuadWithGimbalCameraCfg)
+robot_registry.register("base_quadrotor_with_gimbal_camera_imu", ArticulatedMultirotor, rc.BaseQuadWithGimbalCameraImuCfg)
+robot_registry.register("morphy_compliant_imu", ArticulatedMultirotor, rc.MorphyCompliantImuCfg)
 
 # the reference's package also exports its robot config classes (robots/__init__.py: `from ...base_quad_config import *`, ...)
 globals().update({_k: _v for _k, _v in vars(rc).items() if _k.endswith("Cfg")})

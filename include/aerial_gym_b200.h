@@ -265,6 +265,18 @@ typedef struct AgxArticulation {
  * allocation, no synchronisation. */
 int agx_hp1_articulated_step(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, const AgxArticulation* art, void* stream);
 
+/* agx_hp1_articulated_step, and on the LAST sub-step of the launch the IMU input of body imu_body (in [0, num_bodies)):
+ * imu_input [N,9] out = (f_b (3), n_b (3), w_b (3)), all in body b's frame at that sub-step's start:
+ *   f_b = m_b R_b^T (a_c - g), a_c the classical acceleration of the body's COM: the non-gravitational force on the body, joint
+ *         reactions included (what body_wrench[0:3] is for a rigid robot);
+ *   n_b = I_b R_b^T alpha_b + w_b x I_b w_b, the net torque about the COM (body_wrench[3:6]);
+ *   w_b = R_b^T omega_b, the body's angular velocity in its frame (the stale derived body_angvel).
+ * With physics_steps = 0: f_b = n_b = 0 (agx_hp1_physics_step zeroes body_wrench then) and w_b of the unstepped state.  Every other
+ * output is agx_hp1_articulated_step's, computed by the same source; a separate kernel, so the device's multiply-add contraction may
+ * round it differently (float32 rounding).  Capturable: no allocation, no synchronisation. */
+int agx_hp1_articulated_step_imu(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, const AgxArticulation* art, int imu_body,
+                                 float* imu_input, void* stream);
+
 /* Pose and velocity of every body of an articulated robot, from the root state and art->dof_state (the other [N,...] arrays of
  * `art` are not read).  root_state [N,stride] (stride >= 13, rows as AgxHp1Buffers.root_state); body_state [N,B,13] out, dense,
  * 16-byte aligned, bodies in table order, each row laid out like a root_state row:
