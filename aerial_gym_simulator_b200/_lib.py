@@ -176,6 +176,11 @@ class AgxArticulation(C.Structure):
                 ("dof_velocity_setpoint", fp)]
 
 
+class AgxJointEffort(C.Structure):
+    B = ART_MAX_BODIES
+    _fields_ = [("effort", fp), ("effort_dof", C.c_int32 * B), ("effort_limit", f32 * B)]
+
+
 SENSOR_CAMERA, SENSOR_LIDAR, SENSOR_STEREO_CAMERA, SENSOR_NORMAL_FACEID_CAMERA, SENSOR_NORMAL_FACEID_LIDAR = 0, 1, 2, 3, 4
 
 
@@ -215,6 +220,8 @@ def load():
         "agx_hp1_articulated_step": [C.POINTER(AgxHp1Config), C.POINTER(AgxHp1Buffers), C.POINTER(AgxArticulation), C.c_void_p],
         "agx_hp1_articulated_step_imu": [C.POINTER(AgxHp1Config), C.POINTER(AgxHp1Buffers), C.POINTER(AgxArticulation), C.c_int,
                                          C.c_void_p, C.c_void_p],
+        "agx_hp1_articulated_step_effort": [C.POINTER(AgxHp1Config), C.POINTER(AgxHp1Buffers), C.POINTER(AgxArticulation),
+                                            C.POINTER(AgxJointEffort), C.c_int, C.c_void_p, C.c_void_p],
         "agx_hp1_articulated_body_state": [C.POINTER(AgxArticulation), C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p],
         "agx_hp1_reset": [C.POINTER(AgxHp1Config), C.POINTER(AgxHp1Buffers), C.c_void_p,
                           C.POINTER(AgxHp1ResetDraws), C.c_void_p],
@@ -281,7 +288,7 @@ def load():
         raise AgxError("aux ABI struct size mismatch between _lib.py and libaerial_gym_b200.so")
     if lib.agx_sizeof(0) != C.sizeof(AgxHp1Config) or lib.agx_sizeof(1) != C.sizeof(AgxHp1Buffers) \
             or lib.agx_sizeof(2) != C.sizeof(AgxHp1ResetDraws) or lib.agx_sizeof(10) != C.sizeof(AgxObsGatherPush) \
-            or lib.agx_sizeof(15) != C.sizeof(AgxArticulation):
+            or lib.agx_sizeof(15) != C.sizeof(AgxArticulation) or lib.agx_sizeof(17) != C.sizeof(AgxJointEffort):
         raise AgxError("ABI struct size mismatch between _lib.py and libaerial_gym_b200.so")
     _lib = lib
     return lib

@@ -518,3 +518,14 @@ class MorphyCompliantImuCfg(MorphyCompliantCfg):
     class sensor_config(MorphyCompliantCfg.sensor_config):
         enable_imu = True
         imu_config = BaseLinkImuConfig
+
+
+class BaseQuadWithTorqueGimbalCfg(BaseQuadWithGimbalCameraCfg):
+    """base_quadrotor_with_gimbal_camera with both gimbal joints in effort mode: no implicit drive, the commanded torques of
+    dof_actuation_force_tensor [N, 2] (N m), each clamped to quad_gimbal.urdf's <limit effort> of 0.1 N m.  The camera still rides on
+    gimbal_camera_link; levelling it is the caller's torque law (e.g. a PD on the base's Euler angles)."""
+    class robot_asset(BaseQuadWithGimbalCameraCfg.robot_asset):
+        name = "base_quadrotor_with_torque_gimbal"
+
+    class joint_config(BaseQuadWithGimbalCameraCfg.joint_config):
+        drive_mode = "effort"

@@ -57,6 +57,7 @@ uint64_t agx_sizeof(int which) {
         case 9: return sizeof(AgxE2ERewardParams);
         case 10: return sizeof(AgxObsGatherPush);
         case 15: return sizeof(AgxArticulation);
+        case 17: return sizeof(AgxJointEffort);
 #ifdef AGX_HAVE_HP2
         case 3: return sizeof(AgxHp2Scene);
         case 4: return sizeof(AgxHp2Sensor);

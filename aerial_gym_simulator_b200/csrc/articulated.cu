@@ -79,6 +79,28 @@ ArtImuKernel pick_art_imu_kernel(int M, int B) {
     return B <= 9 ? articulated_step_imu_kernel<8, 9> : articulated_step_imu_kernel<8, AGX_ART_MAX_BODIES>;
 }
 
+// ---- the step with effort-mode joints (agx_hp1_articulated_step_effort): one [D] read of the commanded torques per env and launch,
+// with or without the IMU input
+template <int M, int NB, bool IMU>
+__global__ void __launch_bounds__(kArtThreads)
+articulated_step_effort_kernel(const __grid_constant__ AgxHp1Config cfg, const __grid_constant__ AgxHp1Buffers buf,
+                               const __grid_constant__ AgxArticulation art, const __grid_constant__ AgxJointEffort eff, int imu_body,
+                               float* __restrict__ imu_input) {
+    const int env = blockIdx.x * blockDim.x + threadIdx.x;
+    if (env >= cfg.num_envs) return;
+    art_env_step<M, NB, IMU, true>(cfg, buf, art, env, imu_body, imu_input, &eff);
+}
+
+using ArtEffortKernel = void (*)(const AgxHp1Config, const AgxHp1Buffers, const AgxArticulation, const AgxJointEffort, int, float*);
+template <bool IMU>
+ArtEffortKernel pick_art_effort_kernel_(int M, int B) {
+    if (M == 4) return B <= 9 ? articulated_step_effort_kernel<4, 9, IMU> : articulated_step_effort_kernel<4, AGX_ART_MAX_BODIES, IMU>;
+    return B <= 9 ? articulated_step_effort_kernel<8, 9, IMU> : articulated_step_effort_kernel<8, AGX_ART_MAX_BODIES, IMU>;
+}
+ArtEffortKernel pick_art_effort_kernel(int M, int B, bool imu) {
+    return imu ? pick_art_effort_kernel_<true>(M, B) : pick_art_effort_kernel_<false>(M, B);
+}
+
 // ---- per-body state (agx_hp1_articulated_body_state) ----------------------------------------------------------------------
 // One env per lane, one warp per block.  Each lane builds its env's B rows (13 B floats) in shared memory with art_body_states, the
 // rows of the parents serving as the sweep's scratch, so nothing goes to local memory.  Written straight from the lanes, the rows
@@ -174,4 +196,28 @@ extern "C" int agx_hp1_articulated_step_imu(const AgxHp1Config* cfg, const AgxHp
     pick_art_imu_kernel(cfg->num_motors, art->num_bodies)<<<g, kArtThreads, 0, (cudaStream_t)stream>>>(*cfg, *buf, *art, imu_body,
                                                                                                       imu_input);
     return agx_check_launch("articulated_step_imu_kernel");
+}
+
+extern "C" int agx_hp1_articulated_step_effort(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, const AgxArticulation* art,
+                                               const AgxJointEffort* effort, int imu_body, float* imu_input, void* stream) {
+    int rc = validate_articulation(cfg, buf, art);
+    if (rc) return rc;
+    if (!effort) return agx_set_error(AGX_E_NULL, "effort is NULL");
+    if (imu_input && (imu_body < 0 || imu_body >= art->num_bodies))
+        return agx_set_error(AGX_E_INVALID, "imu_body must be in [0, %d) (got %d)", art->num_bodies, imu_body);
+    bool any = false;
+    for (int i = 1; i < art->num_bodies; ++i) {
+        if (!(effort->effort_limit[i] >= 0.0f))
+            return agx_set_error(AGX_E_INVALID, "effort_limit[%d] must be >= 0 (got %g)", i, (double)effort->effort_limit[i]);
+        if (!effort->effort_dof[i]) continue;
+        if (art->stiffness[i] != 0.0f)
+            return agx_set_error(AGX_E_INVALID, "body %d's joint is in effort mode: it has no implicit drive, stiffness[%d] must be 0", i, i);
+        any = true;
+    }
+    if (cfg->num_envs == 0) return AGX_OK;
+    if (any && !effort->effort) return agx_set_error(AGX_E_NULL, "effort->effort is NULL and a joint is in effort mode");
+    const int g = (cfg->num_envs + kArtThreads - 1) / kArtThreads;
+    pick_art_effort_kernel(cfg->num_motors, art->num_bodies, imu_input != nullptr)<<<g, kArtThreads, 0, (cudaStream_t)stream>>>(
+        *cfg, *buf, *art, *effort, imu_body, imu_input);
+    return agx_check_launch("articulated_step_effort_kernel");
 }

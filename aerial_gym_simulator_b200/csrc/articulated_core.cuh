@@ -172,10 +172,12 @@ AGX_DEV V3 art_body_angvel(const AgxArticulation& art, const EnvState& s, const 
 // The joint drive tau = k (qs - q') + d (qds - qd') is taken at the end-of-step q' = q + dt qd', qd' = qd + dt qdd: its implicit part
 // moves into the joint's pivot D_i = S^T I^A S + dt d + dt^2 k, the explicit part k (qs - q - dt qd) + d (qds - qd) into u_i.
 // IMU: where imu != NULL, also art_imu_input of body imu_body into imu[9]; a0 and qdd are the same either way.
-template <int NB, bool IMU = false>
+// EFFORT: the joints with eff->effort_dof[i] set are torque-driven: qs holds their tau_e and their k is 0, so the explicit force is
+// tau_e - d qd (d = the URDF damping alone, passive) and the pivot S^T I^A S + dt d.
+template <int NB, bool IMU = false, bool EFFORT = false>
 AGX_DEV void art_dynamics(const AgxArticulation& art, const EnvState& s, const float* q, const float* qd, const float* qs,
                           const float* qds, float dt, V3 grav, int M, const float* thrust, V3 F_w, V3 T_w, float* a0, float* qdd,
-                          int imu_body = 0, float* imu = nullptr) {
+                          int imu_body = 0, float* imu = nullptr, const AgxJointEffort* eff = nullptr) {
     const int B = art.num_bodies;
     M33 R[NB];
     V3 P[NB];
@@ -240,7 +242,7 @@ AGX_DEV void art_dynamics(const AgxArticulation& art, const EnvState& s, const f
         const float k = art.stiffness[i], dd = art.damping[i];
         mul66(IA[i], S[i], U[i]);
         const float Dd = sv_dot(S[i], U[i]) + dt * dd + dt * dt * k;
-        const float tau = k * (qs[j] - q[j] - dt * qd[j]) + dd * (qds[j] - qd[j]);
+        const float tau = (EFFORT && eff->effort_dof[i]) ? qs[j] - dd * qd[j] : k * (qs[j] - q[j] - dt * qd[j]) + dd * (qds[j] - qd[j]);
         const float u = tau - sv_dot(S[i], PA[i]);
         const float di = 1.0f / Dd;
         Dinv[i] = di;
@@ -345,9 +347,11 @@ AGX_DEV void art_load_params(const AgxHp1Config& cfg, const AgxHp1Buffers& buf, 
 // Derived states d are those of the last sub-step's start (agx_hp1_physics_step's staleness).
 // IMU: also the IMU input of body imu_body into imu_input [N,9] -- art_imu_input on the last sub-step; with physics_steps = 0,
 // f = n = 0 and w_b of the unstepped state (agx_hp1_physics_step's body_wrench is zero then).  The state arithmetic is unchanged.
-template <int M, int NB, bool IMU = false>
+// EFFORT: the effort DOFs of eff take tau_e = their entry of eff->effort, clamped to +-effort_limit where that is > 0, read once and
+// held in qs for every sub-step (art_dynamics' EFFORT); the other DOFs are stepped as without it.
+template <int M, int NB, bool IMU = false, bool EFFORT = false>
 AGX_DEV void art_env_step(const AgxHp1Config& cfg, const AgxHp1Buffers& buf, const AgxArticulation& art, int env, int imu_body = 0,
-                          float* imu_input = nullptr) {
+                          float* imu_input = nullptr, const AgxJointEffort* eff = nullptr) {
     EnvParams<M> p;
     art_load_params<M>(cfg, buf, env, p);
     const int A = cfg.num_actions;
@@ -364,6 +368,13 @@ AGX_DEV void art_env_step(const AgxHp1Config& cfg, const AgxHp1Buffers& buf, con
         qd[j] = art.dof_state[((size_t)env * D + j) * 2 + 1];
         qs[j] = art.dof_position_setpoint[(size_t)env * D + j];
         qds[j] = art.dof_velocity_setpoint[(size_t)env * D + j];
+    }
+    if constexpr (EFFORT) {
+        for (int j = 0; j < D; ++j) {
+            if (!eff->effort_dof[j + 1]) continue;
+            const float e = eff->effort[(size_t)env * D + j], E = eff->effort_limit[j + 1];
+            qs[j] = E > 0.0f ? fminf(fmaxf(e, -E), E) : e;
+        }
     }
     const V3 grav = ld3c(cfg.gravity);
     Derived d;
@@ -402,7 +413,11 @@ AGX_DEV void art_env_step(const AgxHp1Config& cfg, const AgxHp1Buffers& buf, con
             dtq = dtq + V3{d6[3], d6[4], d6[5]};
         }
         float a0[6];
-        if constexpr (IMU) {
+        if constexpr (EFFORT) {
+            float* imu = (IMU && step + 1 == cfg.physics_steps) ? imu_input + (size_t)env * 9 : nullptr;
+            art_dynamics<NB, IMU, true>(art, s, q, qd, qs, qds, cfg.dt, grav, M, p.thrust, quat_rotate(s.q, df), quat_rotate(s.q, dtq),
+                                        a0, qdd, imu_body, imu, eff);
+        } else if constexpr (IMU) {
             float* imu = (step + 1 == cfg.physics_steps) ? imu_input + (size_t)env * 9 : nullptr;
             art_dynamics<NB, true>(art, s, q, qd, qs, qds, cfg.dt, grav, M, p.thrust, quat_rotate(s.q, df), quat_rotate(s.q, dtq), a0,
                                    qdd, imu_body, imu);

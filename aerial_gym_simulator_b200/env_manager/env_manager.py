@@ -264,6 +264,8 @@ class EnvManager:
             gtd["dof_state_tensor"] = eng.dof_state
             gtd["dof_position_setpoint_tensor"] = eng.dof_position_setpoint
             gtd["dof_velocity_setpoint_tensor"] = eng.dof_velocity_setpoint
+            if getattr(eng, "dof_actuation_force", None) is not None:  # the commanded torques of the effort DOFs, the user's too
+                gtd["dof_actuation_force_tensor"] = eng.dof_actuation_force
             T = lambda v: torch.tensor(np.asarray(v, np.float32), device=dev)
             self._dof_rng = tuple(T(r) for r in (*articulation.init_dof_pos_range, *articulation.init_dof_vel_range))
         # every body's pose and velocity [N,B,13] (rows like robot_state_tensor's, body 0 = the root link), refreshed once per env step

@@ -126,7 +126,10 @@ class MultirotorSpec:
 class ArticulationSpec:
     """The joint layer of an articulated multirotor (DESIGN.md "Articulated robots"): the merged body table of its URDF
     (urdf.ArticulatedBodies), the drive gains per DOF, where each motor sits, and the ranges the joint state is reset to.
-    The MultirotorSpec beside it keeps the zero-configuration mass and inertia, which is what the controller uses."""
+    The MultirotorSpec beside it keeps the zero-configuration mass and inertia, which is what the controller uses.
+    drive_mode: per DOF (a scalar applies to all) "position" -- the implicit drive towards the setpoints -- or "effort" -- no drive
+    (its stiffness and damping are set to 0 here; the URDF <dynamics damping> stays), the engine's dof_actuation_force instead,
+    clamped to +-effort_limit where that is > 0.  effort_limit: [D] N m, default the URDF's <limit effort>."""
 
     bodies: object                     # urdf.ArticulatedBodies
     stiffness: np.ndarray              # [D] k, N m / rad
@@ -137,6 +140,8 @@ class ArticulationSpec:
     motor_torque: np.ndarray           # [M] reaction torque per unit thrust about the motor z axis: -thrust_to_torque_ratio * dir
     init_dof_pos_range: tuple = None   # ([D], [D]) uniform reset range of q; default (0, 0)
     init_dof_vel_range: tuple = None   # ([D], [D]) of q-dot
+    drive_mode: object = "position"    # [D] or scalar: "position" | "effort"
+    effort_limit: np.ndarray = None    # [D] N m, |tau_e| bound of an effort DOF where > 0
 
     def __post_init__(self):
         b, D = self.bodies, self.bodies.num_dofs
@@ -145,6 +150,17 @@ class ArticulationSpec:
         self.damping = np.broadcast_to(np.asarray(self.damping, np.float64), (D,)).copy()
         if (self.stiffness < 0).any() or (self.damping < 0).any():
             raise ValueError("joint stiffness and damping must be >= 0")
+        mode = [self.drive_mode] * D if isinstance(self.drive_mode, str) else list(self.drive_mode)
+        if len(mode) != D or any(m not in ("position", "effort") for m in mode):
+            raise ValueError(f"drive_mode must be 'position' or 'effort', or a list of {D} of them (one per DOF); got {self.drive_mode!r}")
+        self.drive_mode = mode
+        self.effort_dof = np.array([m == "effort" for m in mode], bool)
+        self.effort_limit = np.broadcast_to(np.asarray(b.effort_limit[1:] if self.effort_limit is None else self.effort_limit, np.float64),
+                                            (D,)).copy()
+        if not (self.effort_limit >= 0).all():
+            raise ValueError("effort_limit must be >= 0")
+        self.stiffness[self.effort_dof] = 0.0  # an effort DOF has no implicit drive
+        self.damping[self.effort_dof] = 0.0
         rng = lambda r: (z.copy(), z.copy()) if r is None else tuple(np.broadcast_to(np.asarray(v, np.float64), (D,)).copy() for v in r)
         self.init_dof_pos_range, self.init_dof_vel_range = rng(self.init_dof_pos_range), rng(self.init_dof_vel_range)
         self.motor_body = np.asarray(self.motor_body, np.int64)
@@ -172,12 +188,22 @@ class ArticulationSpec:
                 Ic = R0[k] @ b.inertia[k] @ R0[k].T + b.mass[k] * (float(r @ r) * np.eye(3) - np.outer(r, r))
                 J += float(a @ Ic @ a)
             if not J > 1e-12:
+                why = "it is in effort mode and has no URDF <dynamics damping>" if self.effort_dof[i - 1] else \
+                    "stiffness = damping = 0"
                 raise ValueError(f"joint '{b.joint_names[i]}': its subtree has no inertia about the axis and the joint has no drive "
-                                 "(stiffness = damping = 0), so its acceleration is undefined")
+                                 f"({why}), so its acceleration is undefined")
 
     @property
     def num_dofs(self) -> int:
         return self.bodies.num_dofs
+
+    def effort_struct(self) -> "_lib.AgxJointEffort":
+        """the AgxJointEffort of the effort DOFs (its `effort` pointer left NULL)"""
+        e = _lib.AgxJointEffort()
+        for j in range(self.num_dofs):
+            e.effort_dof[j + 1] = int(self.effort_dof[j])
+            e.effort_limit[j + 1] = float(self.effort_limit[j])
+        return e
 
     def to_struct(self) -> "_lib.AgxArticulation":
         b, a = self.bodies, _lib.AgxArticulation()
@@ -285,7 +311,10 @@ class Hp1Engine:
         step for such a robot.
         imu_body: with an articulation, the body an IMU rides on -- physics_step then runs agx_hp1_articulated_step_imu, which also
         writes imu_input [N,9] = (force f_b, torque n_b, angular velocity w_b) of that body in its own frame, of the last
-        sub-step's start (the IMU's force input; the state update is the same arithmetic)."""
+        sub-step's start (the IMU's force input; the state update is the same arithmetic).
+        An articulation with a DOF in effort mode (ArticulationSpec.drive_mode): the engine also owns dof_actuation_force [N,D],
+        the commanded joint torques, zero until the caller writes them and never written by the engine; physics_step then runs
+        agx_hp1_articulated_step_effort, which reads it in place once per launch (the columns of position DOFs are ignored)."""
         self.lib = _lib.load()
         self.device = torch.device(device)
         if self.device.type != "cuda":
@@ -298,6 +327,7 @@ class Hp1Engine:
         N, M, dev = self.N, self.M, self.device
         self._init_body_state()
         self._init_imu(imu_body)
+        self._init_effort()
         z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=dev)
         self.root_state = z(N, 13)
         self.root_state[:, 6] = 1.0
@@ -393,6 +423,16 @@ class Hp1Engine:
                              "body_wrench (debug_wrench=True)")
         self.imu_body = int(imu_body)
         self.imu_input = torch.zeros(self.N, 9, dtype=torch.float32, device=self.device)
+
+    def _init_effort(self):
+        """dof_actuation_force [N,D] and the AgxJointEffort of an articulated robot with an effort DOF (None otherwise)"""
+        self.dof_actuation_force, self._effort = None, None
+        if self.articulation is None or not self.articulation.effort_dof.any():
+            return
+        self.dof_actuation_force = torch.zeros(self.N, self.articulation.num_dofs, dtype=torch.float32, device=self.device)
+        self._effort = self.articulation.effort_struct()
+        self._effort.effort = self.dof_actuation_force.data_ptr()
+        self._effort_ref = C.byref(self._effort)
 
     def _host_tensor(self, shape, dtype):
         nbytes = max(1, int(np.prod(shape))) * torch.empty((), dtype=dtype).element_size()
@@ -524,6 +564,12 @@ class Hp1Engine:
         self._buf.dist_offset = dist_offset
         if physics_steps is not None:
             self.cfg.physics_steps = int(physics_steps)
+        if self._effort is not None:
+            imu = self.imu_input is not None
+            _lib.check(self.lib.agx_hp1_articulated_step_effort(self._cfg_ref, self._buf_ref, self._art_ref, self._effort_ref,
+                                                                self.imu_body if imu else 0, self._ptr(self.imu_input), self._stream()),
+                       "agx_hp1_articulated_step_effort")
+            return
         if self.imu_input is not None:
             _lib.check(self.lib.agx_hp1_articulated_step_imu(self._cfg_ref, self._buf_ref, self._art_ref, self.imu_body,
                                                              self.imu_input.data_ptr(), self._stream()), "agx_hp1_articulated_step_imu")

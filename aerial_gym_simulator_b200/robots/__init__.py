@@ -106,7 +106,9 @@ class ArticulatedMultirotor(BaseMultirotor):
     """A multirotor whose URDF tree has revolute / continuous joints (DESIGN.md "Articulated robots").  The controller, allocation and
     motor model are BaseMultirotor's, with the zero-configuration mass and inertia; the motors push on the bodies their links were
     merged into, and the joints are driven towards the engine's dof_position_setpoint / dof_velocity_setpoint by the drive of the
-    config's joint_config (stiffness, damping per DOF; a scalar applies to every DOF)."""
+    config's joint_config (stiffness, damping per DOF; a scalar applies to every DOF).  joint_config.drive_mode ("position", the
+    default, or "effort", per DOF or one for all) hands a DOF to the engine's dof_actuation_force instead, clamped to the URDF's
+    <limit effort>."""
     articulated = True
 
     def __init__(self, robot_config, controller_name, env_config, device):
@@ -132,7 +134,7 @@ class ArticulatedMultirotor(BaseMultirotor):
             bodies=b, stiffness=jc.stiffness, damping=jc.damping, motor_body=mb, motor_R=mR, motor_p=mp,
             motor_torque=-cq * np.asarray(ca.motor_directions, np.float64),
             init_dof_pos_range=(jc.min_init_dof_position, jc.max_init_dof_position),
-            init_dof_vel_range=(jc.min_init_dof_velocity, jc.max_init_dof_velocity))
+            init_dof_vel_range=(jc.min_init_dof_velocity, jc.max_init_dof_velocity), drive_mode=getattr(jc, "drive_mode", "position"))
 
 
 for _name, _cfg in (
@@ -150,6 +152,7 @@ robot_registry.register("morphy_compliant", ArticulatedMultirotor, rc.MorphyComp
 robot_registry.register("base_quadrotor_with_gimbal_camera", ArticulatedMultirotor, rc.BaseQuadWithGimbalCameraCfg)
 robot_registry.register("base_quadrotor_with_gimbal_camera_imu", ArticulatedMultirotor, rc.BaseQuadWithGimbalCameraImuCfg)
 robot_registry.register("morphy_compliant_imu", ArticulatedMultirotor, rc.MorphyCompliantImuCfg)
+robot_registry.register("base_quadrotor_with_torque_gimbal", ArticulatedMultirotor, rc.BaseQuadWithTorqueGimbalCfg)
 
 # the reference's package also exports its robot config classes (robots/__init__.py: `from ...base_quad_config import *`, ...)
 globals().update({_k: _v for _k, _v in vars(rc).items() if _k.endswith("Cfg")})

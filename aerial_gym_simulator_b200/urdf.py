@@ -64,6 +64,7 @@ class Joint:
     lower: float = 0.0  # <limit lower upper>
     upper: float = 0.0
     damping: float = 0.0  # <dynamics damping>
+    effort: float = 0.0  # <limit effort>, N m (0: none given)
 
 
 MOVABLE_JOINTS = ("revolute", "continuous")
@@ -90,6 +91,11 @@ class ArticulatedBodies:
     inertia: np.ndarray          # [B,3,3] about the COM, body axes
     link_body: Dict[str, int]    # body each link was merged into
     link_in_body: Dict[str, Tuple[np.ndarray, np.ndarray]]  # (R, p) of each link in its body's frame
+    effort_limit: Optional[np.ndarray] = None  # [B] <limit effort>, N m (0: none; body 0: 0); None = zeros
+
+    def __post_init__(self):
+        if self.effort_limit is None:
+            self.effort_limit = np.zeros(len(self.links))
 
     @property
     def num_bodies(self) -> int:
@@ -163,7 +169,7 @@ class UrdfModel:
         composite_inertia() over the links merged into it.  Joints other than fixed / revolute / continuous, a zero <axis> and more
         than `max_bodies` bodies raise ValueError."""
         by_child = {j.child: j for j in self.joints}
-        names, parent, jn, jk, jR, jp, ax, lo, hi, lim, dmp = [], [], [], [], [], [], [], [], [], [], []
+        names, parent, jn, jk, jR, jp, ax, lo, hi, lim, dmp, eff = [], [], [], [], [], [], [], [], [], [], [], []
         link_body, link_in_body = {}, {}
         for name in self.body_order():
             j = by_child.get(name)
@@ -172,7 +178,7 @@ class UrdfModel:
                     b, T = 0, (np.eye(3), np.zeros(3))
                     names.append(name); parent.append(-1); jn.append(""); jk.append("")
                     jR.append(np.eye(3)); jp.append(np.zeros(3)); ax.append(np.zeros(3))
-                    lo.append(0.0); hi.append(0.0); lim.append(False); dmp.append(0.0)
+                    lo.append(0.0); hi.append(0.0); lim.append(False); dmp.append(0.0); eff.append(0.0)
                 else:
                     b = link_body[j.parent]
                     Rp, pp = link_in_body[j.parent]
@@ -191,6 +197,9 @@ class UrdfModel:
             jR.append(Rp @ j.R); jp.append(pp + Rp @ j.p); ax.append(a / n)
             limited = j.kind == "revolute" and j.lower < j.upper
             lo.append(float(j.lower)); hi.append(float(j.upper)); lim.append(limited); dmp.append(float(j.damping))
+            if not j.effort >= 0:
+                raise ValueError(f"joint '{j.name}' has a negative <limit effort> ({j.effort})")
+            eff.append(float(j.effort))
         B = len(names)
         if B > max_bodies:
             raise ValueError(f"{B} bodies after merging the fixed joints: at most {max_bodies} are supported ({max_bodies - 1} DOFs)")
@@ -211,7 +220,7 @@ class UrdfModel:
             inertia[b] += Rl @ l.inertia @ Rl.T + l.mass * (float(d @ d) * np.eye(3) - np.outer(d, d))
         return ArticulatedBodies(names, np.asarray(parent, np.int64), jn, jk, np.asarray(jR), np.asarray(jp), np.asarray(ax),
                                  np.asarray(lo), np.asarray(hi), np.asarray(lim, bool), np.asarray(dmp), mass, com, inertia,
-                                 link_body, link_in_body)
+                                 link_body, link_in_body, np.asarray(eff, np.float64))
 
 
 def _parse_geometry(el, base_dir) -> Optional[Visual]:
@@ -276,6 +285,7 @@ def parse_urdf(path: str) -> UrdfModel:
             j.axis = _vec(ae.get("xyz"))
         if le is not None:
             j.lower, j.upper = float(le.get("lower", 0.0)), float(le.get("upper", 0.0))
+            j.effort = float(le.get("effort", 0.0))
         if de is not None:
             j.damping = float(de.get("damping", 0.0))
         joints.append(j)

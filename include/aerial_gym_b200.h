@@ -174,7 +174,7 @@ const char* agx_last_error(void);
  * which = 0 AgxHp1Config, 1 AgxHp1Buffers, 2 AgxHp1ResetDraws, 3 AgxHp2Scene, 4 AgxHp2Sensor,
  * 5 AgxNavRewardParams, 6 AgxImuConfig, 7 AgxLidarNavRewardParams, 8 AgxHp2Noise, 9 AgxE2ERewardParams, 10 AgxObsGatherPush,
  * 11 AgxContactParams, 12 AgxContactMotion, 13 AgxObstacleMass, 14 AgxObstacleHull, 15 AgxArticulation,
- * 16 AgxObstacleBoxes */
+ * 16 AgxObstacleBoxes, 17 AgxJointEffort */
 uint64_t agx_sizeof(int which);
 
 /* Host buffers the kernels can address directly (pinned, portable, mapped: cudaHostAlloc).
@@ -276,6 +276,24 @@ int agx_hp1_articulated_step(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, 
  * round it differently (float32 rounding).  Capturable: no allocation, no synchronisation. */
 int agx_hp1_articulated_step_imu(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, const AgxArticulation* art, int imu_body,
                                  float* imu_input, void* stream);
+
+/* Torque-driven joints (effort mode).  Indexed like AgxArticulation's per-body arrays: entry i is body i's joint, DOF i - 1; entry 0
+ * is unused.  An effort DOF has no implicit drive (its AgxArticulation stiffness must be 0; its damping is the URDF <dynamics damping>
+ * alone, a passive -d q-dot); it gets tau_e = clamp(effort[env, i - 1], -effort_limit[i], effort_limit[i]) instead, or the command
+ * unclamped where effort_limit[i] = 0. */
+typedef struct AgxJointEffort {
+    const float* effort;                     /* [N,D] commanded joint torque [N m], read once per launch, held for its sub-steps */
+    int32_t effort_dof[AGX_ART_MAX_BODIES];  /* != 0: body i's joint is in effort mode */
+    float effort_limit[AGX_ART_MAX_BODIES];  /* URDF <limit effort> [N m], >= 0 */
+} AgxJointEffort;
+
+/* agx_hp1_articulated_step (imu_input == NULL) or agx_hp1_articulated_step_imu (imu_input != NULL, imu_body as there) with the
+ * effort-mode joints of `effort`: the joint force u_i of the articulated-body algorithm gains tau_e, an internal torque on the child
+ * body and, in reaction, on its parent.  Position-mode DOFs are stepped exactly as agx_hp1_articulated_step steps them.  A separate
+ * kernel, so the device's multiply-add contraction may round the shared arithmetic differently (float32 rounding).  Capturable: no
+ * allocation, no synchronisation. */
+int agx_hp1_articulated_step_effort(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, const AgxArticulation* art,
+                                    const AgxJointEffort* effort, int imu_body, float* imu_input, void* stream);
 
 /* Pose and velocity of every body of an articulated robot, from the root state and art->dof_state (the other [N,...] arrays of
  * `art` are not read).  root_state [N,stride] (stride >= 13, rows as AgxHp1Buffers.root_state); body_state [N,B,13] out, dense,
