@@ -5,6 +5,7 @@ The .so and the objects under build/ are git-ignored build products."""
 import os
 import subprocess
 import sys
+import sysconfig
 
 PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG, "csrc")
@@ -27,6 +28,9 @@ UNITS = [
     ("hp2_raycast.cu", ["-fmad=false"]),
     ("p2p_allgather.cu", []),
 ]
+# the CPython extension Hp1Engine calls the per-step entry through (csrc/hostcall.cpp): host code only, no device code
+HOSTCALL_SRC = os.path.join(CSRC, "hostcall.cpp")
+HOSTCALL = os.path.join(PKG, "_hostcall" + (sysconfig.get_config_var("EXT_SUFFIX") or ".so"))
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
@@ -51,9 +55,9 @@ def sources():
 
 
 def needs_build():
-    if not os.path.exists(LIB):
+    if not os.path.exists(LIB) or not os.path.exists(HOSTCALL):
         return True
-    t = os.path.getmtime(LIB)
+    t = min(os.path.getmtime(LIB), os.path.getmtime(HOSTCALL))
     deps = [os.path.join(CSRC, f) for f in os.listdir(CSRC)] + [os.path.join(PKG, "..", "include", "aerial_gym_b200.h")]
     return any(os.path.getmtime(d) > t for d in deps if os.path.exists(d))
 
@@ -81,6 +85,12 @@ def build(force=False, verbose=False):
     if r.returncode:
         sys.stderr.write(r.stdout + r.stderr)
         raise RuntimeError("link failed")
+    cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-shared",
+           "-I", sysconfig.get_paths()["include"], HOSTCALL_SRC, "-o", HOSTCALL]
+    r = subprocess.run(cmd, capture_output=True, text=True)
+    if r.returncode:
+        sys.stderr.write(r.stdout + r.stderr)
+        raise RuntimeError("nvcc failed for hostcall.cpp")
     return LIB
 
 

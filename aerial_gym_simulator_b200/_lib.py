@@ -215,6 +215,7 @@ def load():
     for name, args in {
         "agx_hp1_physics_step": [C.POINTER(AgxHp1Config), C.POINTER(AgxHp1Buffers), C.c_void_p],
         "agx_hp1_position_task_step": [C.POINTER(AgxHp1Config), C.POINTER(AgxHp1Buffers), C.c_void_p],
+        "agx_hp1_position_task_step_at": [C.POINTER(AgxHp1Config), C.POINTER(AgxHp1Buffers), C.c_void_p, C.c_uint32],
         "agx_hp1_position_task_step_profiled": [C.POINTER(AgxHp1Config), C.POINTER(AgxHp1Buffers), C.c_void_p,
                                                 C.c_void_p],
         "agx_hp1_articulated_step": [C.POINTER(AgxHp1Config), C.POINTER(AgxHp1Buffers), C.POINTER(AgxArticulation), C.c_void_p],

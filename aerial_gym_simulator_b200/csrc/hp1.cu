@@ -13,6 +13,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#ifdef AGX_TIMELINE
+#include <chrono>
+#endif
 
 #include "../../include/aerial_gym_b200.h"
 #include "agx_common.cuh"
@@ -50,6 +53,9 @@ __device__ __forceinline__ unsigned long long ld_relaxed_gpu_u64(const unsigned 
     unsigned long long v;
     asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
     return v;
+}
+__device__ __forceinline__ void red_relaxed_gpu_add_u32(uint32_t* p, uint32_t v) {
+    asm volatile("red.relaxed.gpu.global.add.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 __device__ __forceinline__ unsigned long long globaltimer_ns() {
     unsigned long long t;
@@ -257,8 +263,9 @@ AGX_HP1_RESET_FN void reset_one_env(const AgxHp1Config& cfg, const AgxHp1Buffers
 // (2) Chained steps.  Env i's step T+1 depends on env i's step T only, so consecutive step launches are
 // chained per TILE, not per grid: launched with programmatic stream serialization, a step's CTAs are
 // scheduled while the previous step's slower warps are still running, each warp takes its step number T
-// from a per-tile claim counter (atomicAdd, before the CTA triggers its dependents, so claims are in launch
-// order), spins until its tile's done-counter says step T-1 has been published (fence.release after the last
+// from the launch (the host counts chained launches: Hp1Engine._chain_T) and counts its claim on a per-tile claim counter with a
+// non-returning reduction -- or, for a caller that does not count (step == kClaimOnDevice), takes T from the claim counter (atomicAdd,
+// before the CTA triggers its dependents, so claims are in launch order) --, spins until its tile's done-counter says step T-1 has been published (fence.release after the last
 // store / relaxed polls, then one fence.acquire before the first L2-only load), and runs.  The launch's tail (slow SMs, the ~6 % of
 // warps with a resetting env) no longer gates the next step.  A warp also waits until step T-2 is complete
 // everywhere, so at most two consecutive steps are in flight and four parity slots suffice:
@@ -275,8 +282,9 @@ AGX_HP1_RESET_FN void reset_one_env(const AgxHp1Config& cfg, const AgxHp1Buffers
 // HOST keeps a step from overwriting a slot whose push has not finished (stream events) -- an in-kernel wait here would let the
 // blocked step's CTAs and their chained successors hold every CTA slot the pending push needs (a deadlock until the wall-clock
 // bound fires: tests/test_gather_protocol_model.py).
-#ifdef AGX_TIMELINE  // debug builds only (tools/dbg/timeline.py): per-warp start / end globaltimer stamps
-__device__ unsigned long long g_timeline[4][8192];
+#ifdef AGX_TIMELINE  // debug builds only (tools/dbg/timeline.py, tools/step_breakdown.py): per-warp globaltimer stamps
+// 0 start, 1 physics done, 2 epilogue done, 3 end; chained steps: 4 step index known (claim), 5 waits done, 6 first loads arrived
+__device__ unsigned long long g_timeline[7][8192];
 __device__ __forceinline__ unsigned long long gtimer() {
     unsigned long long t;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
@@ -290,9 +298,10 @@ __device__ __forceinline__ unsigned long long gtimer() {
 #ifndef AGX_HP1_MIN_BLOCKS
 #define AGX_HP1_MIN_BLOCKS (16 / AGX_HP1_WARPS_PER_BLOCK)  // 16 warps x 128 registers = the register file
 #endif
+constexpr uint32_t kClaimOnDevice = 0xffffffffu;  // `step` of a chained launch whose caller does not count its launches
 template <int M, bool TASK, bool COOP = false, int SPEC = -1>
 __global__ void __launch_bounds__(kThreads, AGX_HP1_MIN_BLOCKS)
-hp1_step_kernel(const __grid_constant__ AgxHp1Config cfg, const __grid_constant__ AgxHp1Buffers buf, int vec_ok) {
+hp1_step_kernel(const __grid_constant__ AgxHp1Config cfg, const __grid_constant__ AgxHp1Buffers buf, int vec_ok, uint32_t step) {
     using SP = HpSpec<SPEC>;
     __shared__ __align__(16) float tiles[kWarpsPerBlock][kTileFloats];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -308,28 +317,40 @@ hp1_step_kernel(const __grid_constant__ AgxHp1Config cfg, const __grid_constant_
     if constexpr (COOP) {
         const int my_tile = blockIdx.x * kWarpsPerBlock + warp;
         const bool has_tile = my_tile < n_tiles;
-        // (The tile's done-counter and the four arrival counters are NOT fetched together with the claim: extra loads on the line the
-        // arrival atomics hammer slow the dependent-chain loop; the acquire spins below touch that line only when they must.)
-        if (has_tile && lane == 0) step_T = atomicAdd(buf.tile_sync + my_tile, 1u);  // claim: which step of this tile am I?
-        step_T = __shfl_sync(0xffffffffu, step_T, 0);
-        __syncthreads();  // every warp of the CTA holds its claim before the CTA lets the next launch in
-        // programmatic dependent launch: once every CTA of this grid is here, the NEXT step's CTAs may be scheduled
-        asm volatile("griddepcontrol.launch_dependents;" ::"r"(step_T) : "memory");
+        if (step != kClaimOnDevice) {
+            // the host knows T: no round trip before the waits, and the next step's CTAs may be scheduled at once (programmatic
+            // dependent launch: once every CTA of this grid is here).  The claim is still counted, so tile_sync reads the same.
+            asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+            step_T = step;
+            if (has_tile && lane == 0) red_relaxed_gpu_add_u32(buf.tile_sync + my_tile, 1u);
+        } else {
+            if (has_tile && lane == 0) step_T = atomicAdd(buf.tile_sync + my_tile, 1u);  // claim: which step of this tile am I?
+            step_T = __shfl_sync(0xffffffffu, step_T, 0);
+            __syncthreads();  // every warp of the CTA holds its claim before the CTA lets the next launch in
+            asm volatile("griddepcontrol.launch_dependents;" ::"r"(step_T) : "memory");
+        }
+        AGX_TL(4);
         if (has_tile) {
             if (lane == 0) {
+                // the tile's previous step has published its state, and step T-2 is complete everywhere (bounds the skew to two steps
+                // in flight).  Both counters are loaded at once, so the common case -- both already satisfied -- costs one round trip.
+                // Only the one arrival counter T selects is read: extra loads on the line the arrival atomics hammer slow the
+                // dependent-chain loop.
                 const uint32_t* done = buf.tile_sync + n_tiles + my_tile;
-                // this tile's previous step has published its state
-                spin_until([&] { return ld_relaxed_gpu_u32(done) == step_T; }, buf.any_reset, 1 | (int)(step_T << 4));
-                if (step_T >= 2u) {  // step T-2 complete everywhere: bounds the skew to two steps in flight
-                    const uint32_t P = step_T - 2u;
-                    const unsigned long long* a2 = reinterpret_cast<const unsigned long long*>(buf.any_reset + 8) + (P & 3u);
-                    const unsigned long long want2 = (unsigned long long)(P / 4u + 1u) * (unsigned long long)n_tiles;
+                const uint32_t P = step_T - 2u;
+                const unsigned long long* a2 = reinterpret_cast<const unsigned long long*>(buf.any_reset + 8) + (P & 3u);
+                const unsigned long long want2 = step_T >= 2u ? (unsigned long long)(P / 4u + 1u) * (unsigned long long)n_tiles : 0ull;
+                const uint32_t done0 = ld_relaxed_gpu_u32(done);
+                const unsigned long long arrived0 = step_T >= 2u ? ld_relaxed_gpu_u64(a2) : 0ull;
+                if (done0 != step_T)
+                    spin_until([&] { return ld_relaxed_gpu_u32(done) == step_T; }, buf.any_reset, 1 | (int)(step_T << 4));
+                if (arrived0 < want2)
                     spin_until([&] { return ld_relaxed_gpu_u64(a2) >= want2; }, buf.any_reset, 2 | (int)(step_T << 4));
-                }
                 fence_acquire_gpu();  // one acquire for both waits, before the warp's first load of the tile
             }
             __syncwarp();
         }
+        AGX_TL(5);
         reset_flag = reinterpret_cast<uint32_t*>(buf.any_reset) + 4 + (step_T & 3u);
         arrive_ctr = reinterpret_cast<unsigned long long*>(buf.any_reset + 8) + (step_T & 3u);
         arrive_target = (unsigned long long)(step_T / 4u + 1u) * (unsigned long long)n_tiles;
@@ -383,6 +404,7 @@ hp1_step_kernel(const __grid_constant__ AgxHp1Config cfg, const __grid_constant_
         // the state is read from the tile only now: its 13 floats are not live across the loads' wait and the ballot above
         if (valid) s = unpack(tile + lane * 13);
         __syncwarp();
+        AGX_TL(6);
         if (valid) {
             // every iteration runs the same instruction sequence, so n fused sub-steps are
             // bit-identical to n single-step launches
@@ -749,7 +771,7 @@ inline int vec_ok_of(const AgxHp1Buffers* buf) {
 #define AGX_HP1_SPEC_LIST(X)
 #endif
 
-using StepKernel = void (*)(const AgxHp1Config, const AgxHp1Buffers, int);
+using StepKernel = void (*)(const AgxHp1Config, const AgxHp1Buffers, int, uint32_t);
 template <bool TASK, bool COOP>
 StepKernel pick_kernel(const AgxHp1Config* cfg) {
     const int id = hp_spec_id(cfg->controller, cfg->flags);
@@ -798,6 +820,77 @@ inline bool hp1_task_step_is_chained(const AgxHp1Config* cfg, const AgxHp1Buffer
     return strict_fused && buf->tile_sync && coop_capacity(pick_kernel<true, true>(cfg)) - kCoopReserve >= grid_for(cfg->num_envs);
 }
 
+// The chained kernel of the task step and whether it is taken, resolved once per shape of (cfg, buf): the flagship enqueues a step every
+// few microseconds, each from the same shape.  Only the shape is remembered; every launch passes the caller's live cfg and buf.
+struct TaskPlan {
+    int num_envs = -1, num_motors = 0, controller = 0, flags = 0;
+    bool tile_sync = false, chained = false;
+    StepKernel coop = nullptr;
+};
+inline const TaskPlan& task_plan(const AgxHp1Config* cfg, const AgxHp1Buffers* buf) {
+    thread_local TaskPlan p;
+    if (p.num_envs != cfg->num_envs || p.num_motors != cfg->num_motors || p.controller != cfg->controller || p.flags != cfg->flags ||
+        p.tile_sync != (buf->tile_sync != nullptr)) {
+        p.num_envs = cfg->num_envs; p.num_motors = cfg->num_motors; p.controller = cfg->controller; p.flags = cfg->flags;
+        p.tile_sync = buf->tile_sync != nullptr;
+        p.coop = pick_kernel<true, true>(cfg);
+        p.chained = hp1_task_step_is_chained(cfg, buf);
+    }
+    return p;
+}
+cudaLaunchAttribute* chained_attr() {
+    static cudaLaunchAttribute a = [] {
+        cudaLaunchAttribute x = {};
+        x.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+        x.val.programmaticStreamSerializationAllowed = 1;
+        return x;
+    }();
+    return &a;
+}
+
+// the fused task step; step = T of a chained launch, or kClaimOnDevice
+int task_step(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, void* stream, void* ev_after_main, uint32_t step) {
+    int rc = validate(cfg, buf, true);
+    if (rc) return rc;
+    if (cfg->num_envs == 0) return AGX_OK;
+    cudaStream_t st = (cudaStream_t)stream;
+    int g = grid_for(cfg->num_envs), v = vec_ok_of(buf);
+    const TaskPlan& plan = task_plan(cfg, buf);
+    if (plan.chained && !ev_after_main) {
+        // single launch: the whole grid is resident at once (g <= occupancy x SMs), so the in-kernel
+        // one-sided barrier cannot starve -- no cooperative-launch API needed for that
+        cudaLaunchConfig_t lc = {};
+        lc.gridDim = dim3(g);
+        lc.blockDim = dim3(kThreads);
+        lc.stream = st;
+        lc.attrs = chained_attr();
+        lc.numAttrs = 1;
+        cudaError_t e = cudaLaunchKernelEx(&lc, plan.coop, *cfg, *buf, v, step);
+        return agx_check_cuda(e, "hp1_step_kernel<task, single-launch>");
+    }
+    const bool strict_fused = (cfg->flags & AGX_F_DEVICE_RNG_RESET) && (cfg->flags & AGX_F_STRICT_STALE_OBS);
+    const bool derived = buf->euler || buf->vehicle_orientation || buf->vehicle_linvel || buf->body_linvel || buf->body_angvel;
+    pick_kernel<true, false>(cfg)<<<g, kThreads, 0, st>>>(*cfg, *buf, v, 0u);
+    rc = agx_check_launch("hp1_step_kernel<task>");
+    if (rc) return rc;
+    if (ev_after_main) {
+        rc = agx_check_cuda(cudaEventRecord((cudaEvent_t)ev_after_main, st), "cudaEventRecord");
+        if (rc) return rc;
+    }
+    // stale-derived-state quirk (SURVEY 3.1): if ANY env reset this step the reference refreshes
+    // the derived states of ALL envs before the observation is read (base_multirotor.py:204-205).
+    if (strict_fused) {
+        if (buf->fresh_vel && !derived) {
+            hp1_obs_patch_kernel<<<(cfg->num_envs + 255) / 256, 256, 0, st>>>(cfg->num_envs, buf->fresh_vel, buf->obs, buf->any_reset);
+            rc = agx_check_launch("hp1_obs_patch_kernel");
+        } else {
+            hp1_refresh_kernel<<<g, kThreads, 0, st>>>(*cfg, *buf, 1, v);
+            rc = agx_check_launch("hp1_refresh_kernel");
+        }
+    }
+    return rc;
+}
+
 }  // namespace
 
 extern "C" {
@@ -837,6 +930,33 @@ int agx_hp1_check(const AgxHp1Buffers* buf, void* stream) {
 int agx_dbg_timeline(unsigned long long* host_out) {
     return agx_check_cuda(cudaMemcpyFromSymbol(host_out, g_timeline, sizeof(g_timeline)), "timeline");
 }
+__global__ void dbg_empty_full_params(const __grid_constant__ AgxHp1Config, const __grid_constant__ AgxHp1Buffers, int, uint32_t) {}
+__global__ void dbg_empty_buf_params(const __grid_constant__ AgxHp1Buffers) {}
+// host microseconds per call, n calls each: out[0] the task-step entry up to its launch (validation, plan), out[1] cudaLaunchKernelEx
+// of an empty kernel with the chained step's launch configuration and parameter block, out[2] the same with AgxHp1Buffers alone
+int agx_dbg_host_costs(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, void* stream, int n, double* out) {
+    using clk = std::chrono::steady_clock;
+    const auto us = [n](clk::time_point a, clk::time_point b) { return std::chrono::duration<double, std::micro>(b - a).count() / n; };
+    volatile int sink = 0;
+    auto t0 = clk::now();
+    for (int i = 0; i < n; ++i) {
+        int rc = validate(cfg, buf, true);
+        sink = sink + rc + (int)task_plan(cfg, buf).chained + grid_for(cfg->num_envs) + vec_ok_of(buf);
+    }
+    auto t1 = clk::now();
+    cudaLaunchConfig_t lc = {};
+    lc.gridDim = dim3(grid_for(cfg->num_envs));
+    lc.blockDim = dim3(kThreads);
+    lc.stream = (cudaStream_t)stream;
+    lc.attrs = chained_attr();
+    lc.numAttrs = 1;
+    for (int i = 0; i < n; ++i) cudaLaunchKernelEx(&lc, dbg_empty_full_params, *cfg, *buf, 1, (uint32_t)i);
+    auto t2 = clk::now();
+    for (int i = 0; i < n; ++i) cudaLaunchKernelEx(&lc, dbg_empty_buf_params, *buf);
+    auto t3 = clk::now();
+    out[0] = us(t0, t1); out[1] = us(t1, t2); out[2] = us(t2, t3);
+    return agx_check_cuda(cudaStreamSynchronize((cudaStream_t)stream), "agx_dbg_host_costs");
+}
 #endif
 
 int agx_hp1_physics_step(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, void* stream) {
@@ -845,7 +965,7 @@ int agx_hp1_physics_step(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, void
     if (cfg->num_envs == 0) return AGX_OK;
     cudaStream_t st = (cudaStream_t)stream;
     int g = grid_for(cfg->num_envs), v = vec_ok_of(buf);
-    pick_kernel<false, false>(cfg)<<<g, kThreads, 0, st>>>(*cfg, *buf, v);
+    pick_kernel<false, false>(cfg)<<<g, kThreads, 0, st>>>(*cfg, *buf, v, 0u);
     return agx_check_launch("hp1_step_kernel");
 }
 
@@ -864,47 +984,12 @@ int agx_hp1_position_task_step_gathered(const AgxHp1Config* cfg, const AgxHp1Buf
 
 int agx_hp1_position_task_step_profiled(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, void* stream,
                                         void* ev_after_main) {
-    int rc = validate(cfg, buf, true);
-    if (rc) return rc;
-    if (cfg->num_envs == 0) return AGX_OK;
-    cudaStream_t st = (cudaStream_t)stream;
-    int g = grid_for(cfg->num_envs), v = vec_ok_of(buf);
-    const bool strict_fused = (cfg->flags & AGX_F_DEVICE_RNG_RESET) && (cfg->flags & AGX_F_STRICT_STALE_OBS);
-    const bool derived = buf->euler || buf->vehicle_orientation || buf->vehicle_linvel || buf->body_linvel || buf->body_angvel;
-    if (hp1_task_step_is_chained(cfg, buf) && !ev_after_main) {
-        // single launch: the whole grid is resident at once (g <= occupancy x SMs), so the in-kernel
-        // one-sided barrier cannot starve -- no cooperative-launch API needed for that
-        cudaLaunchConfig_t lc = {};
-        lc.gridDim = dim3(g);
-        lc.blockDim = dim3(kThreads);
-        lc.stream = st;
-        cudaLaunchAttribute at[1];
-        at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        at[0].val.programmaticStreamSerializationAllowed = 1;
-        lc.attrs = at;
-        lc.numAttrs = 1;
-        cudaError_t e = cudaLaunchKernelEx(&lc, pick_kernel<true, true>(cfg), *cfg, *buf, v);
-        return agx_check_cuda(e, "hp1_step_kernel<task, single-launch>");
-    }
-    pick_kernel<true, false>(cfg)<<<g, kThreads, 0, st>>>(*cfg, *buf, v);
-    rc = agx_check_launch("hp1_step_kernel<task>");
-    if (rc) return rc;
-    if (ev_after_main) {
-        rc = agx_check_cuda(cudaEventRecord((cudaEvent_t)ev_after_main, st), "cudaEventRecord");
-        if (rc) return rc;
-    }
-    // stale-derived-state quirk (SURVEY 3.1): if ANY env reset this step the reference refreshes
-    // the derived states of ALL envs before the observation is read (base_multirotor.py:204-205).
-    if (strict_fused) {
-        if (buf->fresh_vel && !derived) {
-            hp1_obs_patch_kernel<<<(cfg->num_envs + 255) / 256, 256, 0, st>>>(cfg->num_envs, buf->fresh_vel, buf->obs, buf->any_reset);
-            rc = agx_check_launch("hp1_obs_patch_kernel");
-        } else {
-            hp1_refresh_kernel<<<g, kThreads, 0, st>>>(*cfg, *buf, 1, v);
-            rc = agx_check_launch("hp1_refresh_kernel");
-        }
-    }
-    return rc;
+    return task_step(cfg, buf, stream, ev_after_main, kClaimOnDevice);
+}
+
+int agx_hp1_position_task_step_at(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, void* stream, uint32_t step_index) {
+    if (step_index == kClaimOnDevice) return agx_set_error(AGX_E_INVALID, "step_index 0xffffffff is reserved");
+    return task_step(cfg, buf, stream, nullptr, step_index);
 }
 
 int agx_hp1_reset(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, const uint8_t* mask, const AgxHp1ResetDraws* draws,

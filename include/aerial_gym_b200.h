@@ -200,6 +200,12 @@ int agx_hp1_physics_step(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, void
  * envs to reset are only flagged (reset_mask, any_reset[0]) and the caller follows with
  * agx_hp1_reset + agx_hp1_refresh. */
 int agx_hp1_position_task_step(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, void* stream);
+/* Same call for a caller that counts its chained launches: step_index = T, the number of launches of (cfg, buf) that took the
+ * single-launch path (agx_hp1_task_step_is_chained) since tile_sync / any_reset were zeroed.  agx_hp1_position_task_step learns T
+ * from a per-tile claim counter, one device round trip before each warp can wait for its tile; this call hands it to the kernel, which
+ * still counts the claim (tile_sync reads the same after either call).  A wrong T leaves a wait to time out (AGX_E_TIMEOUT).
+ * step_index 0xffffffff is refused (AGX_E_INVALID); it is ignored on the two-launch path. */
+int agx_hp1_position_task_step_at(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, void* stream, uint32_t step_index);
 /* The chained step with its observation gather in ONE call (three launches, one host round trip -- at ~10 us per step the host's
  * launch path is the next bottleneck): agx_obs_gather_gate(gate_read_done, gate_need_epoch) on `stream` unless gate_read_done is
  * NULL, agx_hp1_position_task_step(cfg, buf, stream), agx_obs_gather_push(push, push_stream).  See those three. */

@@ -1,4 +1,4 @@
-"""Per-warp timeline of the cooperative HP1 step (debug build, tools/dbg/build_timeline.sh):
+"""Per-warp timeline of the cooperative HP1 step (debug build: python tools/build_variant.py timeline --hp1 "-DAGX_TIMELINE"):
     AGX_LIB_PATH=tools/dbg/libagx_timeline.so python tools/dbg/timeline.py"""
 import ctypes as C
 import sys
@@ -25,7 +25,7 @@ lib.agx_dbg_timeline.argtypes = [C.c_void_p]
 for i in range(64):
     engs[i % R].position_task_step(acts[i % 8])
 torch.cuda.synchronize()
-out = np.zeros((4, 8192), dtype=np.uint64)
+out = np.zeros((7, 8192), dtype=np.uint64)  # g_timeline[7][8192] (hp1.cu)
 W = (N + 31) // 32
 rows = []
 NREP = int(sys.argv[2]) if len(sys.argv) > 2 else 5
