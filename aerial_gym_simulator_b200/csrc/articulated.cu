@@ -101,6 +101,80 @@ ArtEffortKernel pick_art_effort_kernel(int M, int B, bool imu) {
     return imu ? pick_art_effort_kernel_<true>(M, B) : pick_art_effort_kernel_<false>(M, B);
 }
 
+// ---- the step with the joint forces (agx_hp1_articulated_step_joint_force): the effort kernel's arithmetic plus the rows of
+// joint_wrench [N,B,6] and dof_force [N,D] on the last sub-step.  The IMU input and the effort DOFs are resolved at run time (a NULL
+// imu_input, an effort table without effort DOFs), so four instantiations cover every robot.  Written straight from the lanes, a
+// warp's rows would sit (6 B + D) floats apart and no store would coalesce; instead each lane's art_dynamics writes its env's rows
+// into shared memory (6 B + D floats, plus one when that is even, so that the 32 lanes' accesses at the same offset fall in 32
+// different banks), and the warp then copies its contiguous spans of joint_wrench and dof_force out with 16-byte stores, as
+// articulated_body_state_kernel does.
+constexpr int kWarp = 32;
+
+// out[0, n len) = the rows [n][len] of a warp's lanes, lane e's at s + e st + off; out 16-byte aligned
+__device__ void copy_warp_rows(float* __restrict__ out, const float* s, int st, int off, int len, int n, int lane) {
+    const int total = n * len, n4 = total >> 2;
+    for (int k = lane; k < n4; k += kWarp) {
+        float v[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int g = 4 * k + j, e = g / len;
+            v[j] = s[e * st + off + g - e * len];
+        }
+        reinterpret_cast<float4*>(out)[k] = make_float4(v[0], v[1], v[2], v[3]);
+    }
+    for (int g = 4 * n4 + lane; g < total; g += kWarp) {
+        const int e = g / len;
+        out[g] = s[e * st + off + g - e * len];
+    }
+}
+
+// floats of one lane's rows in shared memory: 6 B + D, made odd
+inline __host__ __device__ int joint_force_row_stride(int B) { return (7 * B - 1) | 1; }
+
+template <int M, int NB>
+__global__ void __launch_bounds__(kArtThreads)
+articulated_step_joint_force_kernel(const __grid_constant__ AgxHp1Config cfg, const __grid_constant__ AgxHp1Buffers buf,
+                                    const __grid_constant__ AgxArticulation art, const __grid_constant__ AgxJointEffort eff,
+                                    int imu_body, float* __restrict__ imu_input, float* __restrict__ joint_wrench,
+                                    float* __restrict__ dof_force) {
+    extern __shared__ float s_joint_rows[];
+    const int lane = threadIdx.x % kWarp;
+    const int env0 = blockIdx.x * blockDim.x + threadIdx.x - lane;
+    if (env0 >= cfg.num_envs) return;  // whole warps only: the rest of the warp copies below
+    const int B = art.num_bodies, D = art.num_dofs, W = 6 * B, st = joint_force_row_stride(B);
+    float* s_warp = s_joint_rows + (threadIdx.x - lane) * st;
+    const int env = env0 + lane;
+    if (env < cfg.num_envs)
+        art_env_step<M, NB, true, true, true>(cfg, buf, art, env, imu_body, imu_input, &eff, s_warp + lane * st, s_warp + lane * st + W);
+    __syncwarp();
+    const int n = min(kWarp, cfg.num_envs - env0);
+    copy_warp_rows(joint_wrench + (size_t)env0 * W, s_warp, st, 0, W, n, lane);  // 16-byte aligned: env0 W is a multiple of 32 x 6
+    if (D) copy_warp_rows(dof_force + (size_t)env0 * D, s_warp, st, W, D, n, lane);
+}
+
+using ArtJointForceKernel = void (*)(const AgxHp1Config, const AgxHp1Buffers, const AgxArticulation, const AgxJointEffort, int, float*,
+                                     float*, float*);
+ArtJointForceKernel pick_art_joint_force_kernel(int M, int B) {
+    if (M == 4) return B <= 9 ? articulated_step_joint_force_kernel<4, 9> : articulated_step_joint_force_kernel<4, AGX_ART_MAX_BODIES>;
+    return B <= 9 ? articulated_step_joint_force_kernel<8, 9> : articulated_step_joint_force_kernel<8, AGX_ART_MAX_BODIES>;
+}
+
+// the checks of an effort table against art; its command array only where a DOF is in effort mode and there are envs
+int validate_effort(const AgxHp1Config* cfg, const AgxArticulation* art, const AgxJointEffort* effort) {
+    bool any = false;
+    for (int i = 1; i < art->num_bodies; ++i) {
+        if (!(effort->effort_limit[i] >= 0.0f))
+            return agx_set_error(AGX_E_INVALID, "effort_limit[%d] must be >= 0 (got %g)", i, (double)effort->effort_limit[i]);
+        if (!effort->effort_dof[i]) continue;
+        if (art->stiffness[i] != 0.0f)
+            return agx_set_error(AGX_E_INVALID, "body %d's joint is in effort mode: it has no implicit drive, stiffness[%d] must be 0", i, i);
+        any = true;
+    }
+    if (cfg->num_envs > 0 && any && !effort->effort)
+        return agx_set_error(AGX_E_NULL, "effort->effort is NULL and a joint is in effort mode");
+    return AGX_OK;
+}
+
 // ---- per-body state (agx_hp1_articulated_body_state) ----------------------------------------------------------------------
 // One env per lane, one warp per block.  Each lane builds its env's B rows (13 B floats) in shared memory with art_body_states, the
 // rows of the parents serving as the sweep's scratch, so nothing goes to local memory.  Written straight from the lanes, the rows
@@ -205,19 +279,35 @@ extern "C" int agx_hp1_articulated_step_effort(const AgxHp1Config* cfg, const Ag
     if (!effort) return agx_set_error(AGX_E_NULL, "effort is NULL");
     if (imu_input && (imu_body < 0 || imu_body >= art->num_bodies))
         return agx_set_error(AGX_E_INVALID, "imu_body must be in [0, %d) (got %d)", art->num_bodies, imu_body);
-    bool any = false;
-    for (int i = 1; i < art->num_bodies; ++i) {
-        if (!(effort->effort_limit[i] >= 0.0f))
-            return agx_set_error(AGX_E_INVALID, "effort_limit[%d] must be >= 0 (got %g)", i, (double)effort->effort_limit[i]);
-        if (!effort->effort_dof[i]) continue;
-        if (art->stiffness[i] != 0.0f)
-            return agx_set_error(AGX_E_INVALID, "body %d's joint is in effort mode: it has no implicit drive, stiffness[%d] must be 0", i, i);
-        any = true;
-    }
+    if ((rc = validate_effort(cfg, art, effort))) return rc;
     if (cfg->num_envs == 0) return AGX_OK;
-    if (any && !effort->effort) return agx_set_error(AGX_E_NULL, "effort->effort is NULL and a joint is in effort mode");
     const int g = (cfg->num_envs + kArtThreads - 1) / kArtThreads;
     pick_art_effort_kernel(cfg->num_motors, art->num_bodies, imu_input != nullptr)<<<g, kArtThreads, 0, (cudaStream_t)stream>>>(
         *cfg, *buf, *art, *effort, imu_body, imu_input);
     return agx_check_launch("articulated_step_effort_kernel");
+}
+
+extern "C" int agx_hp1_articulated_step_joint_force(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, const AgxArticulation* art,
+                                                    const AgxJointEffort* effort, int imu_body, float* imu_input, float* joint_wrench,
+                                                    float* dof_force, void* stream) {
+    int rc = validate_articulation(cfg, buf, art);
+    if (rc) return rc;
+    if (effort && (rc = validate_effort(cfg, art, effort))) return rc;
+    if (imu_input && (imu_body < 0 || imu_body >= art->num_bodies))
+        return agx_set_error(AGX_E_INVALID, "imu_body must be in [0, %d) (got %d)", art->num_bodies, imu_body);
+    if (cfg->num_envs == 0) return AGX_OK;
+    if (!joint_wrench || (art->num_dofs > 0 && !dof_force)) return agx_set_error(AGX_E_NULL, "joint_wrench/dof_force is NULL");
+    if (((uintptr_t)joint_wrench | (uintptr_t)dof_force) & 15)
+        return agx_set_error(AGX_E_INVALID, "joint_wrench and dof_force must be 16-byte aligned");
+    AgxJointEffort none = {};  // no effort DOF: every joint is stepped as agx_hp1_articulated_step steps it
+    const int g = (cfg->num_envs + kArtThreads - 1) / kArtThreads;
+    const ArtJointForceKernel kern = pick_art_joint_force_kernel(cfg->num_motors, art->num_bodies);
+    const size_t smem = sizeof(float) * kArtThreads * joint_force_row_stride(art->num_bodies);  // <= 56.8 KB at 16 bodies
+    if (smem > 48 * 1024) {
+        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) return agx_set_error(AGX_E_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
+    }
+    kern<<<g, kArtThreads, smem, (cudaStream_t)stream>>>(*cfg, *buf, *art, effort ? *effort : none, imu_body, imu_input, joint_wrench,
+                                                          dof_force);
+    return agx_check_launch("articulated_step_joint_force_kernel");
 }

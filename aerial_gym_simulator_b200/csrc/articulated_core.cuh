@@ -146,6 +146,24 @@ AGX_DEV void art_imu_input(const AgxArticulation& art, int b, const M33& R, V3 P
     out[6] = wb.x; out[7] = wb.y; out[8] = wb.z;
 }
 
+// ---- the joint force of one body (agx_hp1_articulated_step_joint_force) ------------------------------------------------------
+// After the ABA's backward pass, body i's articulated inertia I^A and bias force p^A are final (only its ancestors' are still summed
+// into), and the forward pass gives its acceleration A; f = I^A A + p^A = (n_O; F) is the spatial force the parent exerts on the
+// subtree of body i through joint i, world axes about O.  out [6] = (R^T F, R^T (n_O - P x F)): the force, then the torque about the
+// joint origin P, both in body i's frame; *dof = axis_i . (that torque) = S_i^T f, the joint torque of the implicit drive at the
+// unprojected end-of-step state (DESIGN.md "Joint force sensing").
+AGX_DEV void art_joint_force(const AgxArticulation& art, int i, const M33& R, V3 P, const float* IA, const float* PA, const float* A,
+                             float* out, float* dof) {
+    float f[6];
+    mul66(IA, A, f);
+    const V3 Fw{f[3] + PA[3], f[4] + PA[4], f[5] + PA[5]};
+    const V3 nw{f[0] + PA[0], f[1] + PA[1], f[2] + PA[2]};
+    const V3 F = mul33tv(R, Fw), n = mul33tv(R, nw - cross(P, Fw));
+    out[0] = F.x; out[1] = F.y; out[2] = F.z;
+    out[3] = n.x; out[4] = n.y; out[5] = n.z;
+    *dof = dot(ld3(art.axis[i]), n);
+}
+
 // w_b = R_b^T w_b of body b without the dynamics (the IMU input of a launch with physics_steps = 0): the forward kinematics of
 // art_dynamics along the bodies 0..b
 template <int NB>
@@ -174,10 +192,12 @@ AGX_DEV V3 art_body_angvel(const AgxArticulation& art, const EnvState& s, const 
 // IMU: where imu != NULL, also art_imu_input of body imu_body into imu[9]; a0 and qdd are the same either way.
 // EFFORT: the joints with eff->effort_dof[i] set are torque-driven: qs holds their tau_e and their k is 0, so the explicit force is
 // tau_e - d qd (d = the URDF damping alone, passive) and the pivot S^T I^A S + dt d.
-template <int NB, bool IMU = false, bool EFFORT = false>
+// JFORCE: where jw != NULL, also art_joint_force of every body i >= 1 into jw + 6 i and jdof + i - 1, and zeros into jw[0..5].
+template <int NB, bool IMU = false, bool EFFORT = false, bool JFORCE = false>
 AGX_DEV void art_dynamics(const AgxArticulation& art, const EnvState& s, const float* q, const float* qd, const float* qs,
                           const float* qds, float dt, V3 grav, int M, const float* thrust, V3 F_w, V3 T_w, float* a0, float* qdd,
-                          int imu_body = 0, float* imu = nullptr, const AgxJointEffort* eff = nullptr) {
+                          int imu_body = 0, float* imu = nullptr, const AgxJointEffort* eff = nullptr, float* jw = nullptr,
+                          float* jdof = nullptr) {
     const int B = art.num_bodies;
     M33 R[NB];
     V3 P[NB];
@@ -277,6 +297,15 @@ AGX_DEV void art_dynamics(const AgxArticulation& art, const EnvState& s, const f
         qdd[i - 1] = x;
 #pragma unroll
         for (int r = 0; r < 6; ++r) A[i][r] = ai[r] + S[i][r] * x;
+        if constexpr (JFORCE) {
+            if (jw) art_joint_force(art, i, R[i], P[i], IA[i], PA[i], A[i], jw + 6 * i, jdof + (i - 1));
+        }
+    }
+    if constexpr (JFORCE) {
+        if (jw) {
+#pragma unroll
+            for (int r = 0; r < 6; ++r) jw[r] = 0.0f;
+        }
     }
     if constexpr (IMU) {
         if (imu) art_imu_input(art, imu_body, R[imu_body], P[imu_body], V[imu_body], A[imu_body], grav, imu);
@@ -349,9 +378,13 @@ AGX_DEV void art_load_params(const AgxHp1Config& cfg, const AgxHp1Buffers& buf, 
 // f = n = 0 and w_b of the unstepped state (agx_hp1_physics_step's body_wrench is zero then).  The state arithmetic is unchanged.
 // EFFORT: the effort DOFs of eff take tau_e = their entry of eff->effort, clamped to +-effort_limit where that is > 0, read once and
 // held in qs for every sub-step (art_dynamics' EFFORT); the other DOFs are stepped as without it.
-template <int M, int NB, bool IMU = false, bool EFFORT = false>
+// JFORCE (with IMU and EFFORT): also the joint forces of the last sub-step into THIS env's rows, joint_wrench [B,6] and
+// dof_force [D] (art_dynamics' JFORCE; the kernel points them at shared memory), both zero with physics_steps = 0.  The IMU input is written only where imu_input != NULL, and an eff
+// without effort DOFs steps every DOF as the plain step does.  The state arithmetic is unchanged.
+template <int M, int NB, bool IMU = false, bool EFFORT = false, bool JFORCE = false>
 AGX_DEV void art_env_step(const AgxHp1Config& cfg, const AgxHp1Buffers& buf, const AgxArticulation& art, int env, int imu_body = 0,
-                          float* imu_input = nullptr, const AgxJointEffort* eff = nullptr) {
+                          float* imu_input = nullptr, const AgxJointEffort* eff = nullptr, float* joint_wrench = nullptr,
+                          float* dof_force = nullptr) {
     EnvParams<M> p;
     art_load_params<M>(cfg, buf, env, p);
     const int A = cfg.num_actions;
@@ -413,7 +446,13 @@ AGX_DEV void art_env_step(const AgxHp1Config& cfg, const AgxHp1Buffers& buf, con
             dtq = dtq + V3{d6[3], d6[4], d6[5]};
         }
         float a0[6];
-        if constexpr (EFFORT) {
+        if constexpr (JFORCE) {
+            const bool last = step + 1 == cfg.physics_steps;
+            float* imu = (last && imu_input) ? imu_input + (size_t)env * 9 : nullptr;
+            art_dynamics<NB, true, true, true>(art, s, q, qd, qs, qds, cfg.dt, grav, M, p.thrust, quat_rotate(s.q, df),
+                                               quat_rotate(s.q, dtq), a0, qdd, imu_body, imu, eff, last ? joint_wrench : nullptr,
+                                               dof_force);
+        } else if constexpr (EFFORT) {
             float* imu = (IMU && step + 1 == cfg.physics_steps) ? imu_input + (size_t)env * 9 : nullptr;
             art_dynamics<NB, IMU, true>(art, s, q, qd, qs, qds, cfg.dt, grav, M, p.thrust, quat_rotate(s.q, df), quat_rotate(s.q, dtq),
                                         a0, qdd, imu_body, imu, eff);
@@ -427,8 +466,14 @@ AGX_DEV void art_env_step(const AgxHp1Config& cfg, const AgxHp1Buffers& buf, con
         art_integrate(cfg, art, s, a0, q, qd, qdd);
     }
     if (cfg.physics_steps == 0) d = update_states(s);
-    if constexpr (IMU) {
+    if constexpr (JFORCE) {
         if (cfg.physics_steps == 0) {
+            for (int k = 0; k < 6 * art.num_bodies; ++k) joint_wrench[k] = 0.0f;
+            for (int j = 0; j < D; ++j) dof_force[j] = 0.0f;
+        }
+    }
+    if constexpr (IMU) {
+        if (cfg.physics_steps == 0 && (!JFORCE || imu_input)) {
             const V3 wb = art_body_angvel<NB>(art, s, q, qd, imu_body);
             float* o = imu_input + (size_t)env * 9;
             o[0] = 0.0f; o[1] = 0.0f; o[2] = 0.0f; o[3] = 0.0f; o[4] = 0.0f; o[5] = 0.0f;

@@ -251,6 +251,9 @@ class EnvManager:
         extra = {"articulation": articulation} if articulation is not None else {}
         if articulation is not None and imu_on:
             extra["imu_body"] = self._imu_link[1]  # the step also writes that body's force input (Hp1Engine.imu_input)
+        # joint force sensing (Isaac Gym's enable_dof_force_sensors): the step also writes every joint's wrench and DOF force
+        if getattr(getattr(self.robot_cfg, "joint_config", None), "enable_dof_force_sensors", False):
+            extra["joint_force"] = True
         self.engine = Hp1Engine(
             spec, N, dev, physics_steps=1, seed=int(self.env_args.get("seed", 0)),
             env_id_offset=int(self.env_args.get("env_id_offset", 0)), device_rng_reset=(self.reset_rng == "device"),
@@ -266,6 +269,9 @@ class EnvManager:
             gtd["dof_velocity_setpoint_tensor"] = eng.dof_velocity_setpoint
             if getattr(eng, "dof_actuation_force", None) is not None:  # the commanded torques of the effort DOFs, the user's too
                 gtd["dof_actuation_force_tensor"] = eng.dof_actuation_force
+            if getattr(eng, "dof_force", None) is not None:  # written by every step, rows of the wrench in robot_body_names order
+                gtd["dof_force_tensor"] = eng.dof_force
+                gtd["robot_joint_wrench_tensor"] = eng.joint_wrench
             T = lambda v: torch.tensor(np.asarray(v, np.float32), device=dev)
             self._dof_rng = tuple(T(r) for r in (*articulation.init_dof_pos_range, *articulation.init_dof_vel_range))
         # every body's pose and velocity [N,B,13] (rows like robot_state_tensor's, body 0 = the root link), refreshed once per env step

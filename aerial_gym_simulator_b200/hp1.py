@@ -306,7 +306,7 @@ class Hp1Engine:
     def __init__(self, spec: MultirotorSpec, num_envs: int, device="cuda:0", *, physics_steps=1,
                  episode_len_steps=500, seed=0, env_id_offset=0, device_rng_reset=True, strict_stale_obs=True,
                  materialize_derived=True, per_env_params="auto", debug_wrench=False, host_io=False, articulation=None,
-                 imu_body=None):
+                 imu_body=None, joint_force=False):
         """host_io: obs / reward / terminations / truncations live in pinned, device-mapped HOST
         memory (agx_host_alloc) and the fused task step stores them there directly over PCIe;
         `actions` may then be a pinned host tensor (e.g. `self.host_actions`) that the kernel
@@ -320,7 +320,11 @@ class Hp1Engine:
         sub-step's start (the IMU's force input; the state update is the same arithmetic).
         An articulation with a DOF in effort mode (ArticulationSpec.drive_mode): the engine also owns dof_actuation_force [N,D],
         the commanded joint torques, zero until the caller writes them and never written by the engine; physics_step then runs
-        agx_hp1_articulated_step_effort, which reads it in place once per launch (the columns of position DOFs are ignored)."""
+        agx_hp1_articulated_step_effort, which reads it in place once per launch (the columns of position DOFs are ignored).
+        joint_force: with an articulation, the engine also owns joint_wrench [N,B,6] and dof_force [N,D], zero until the first step;
+        physics_step then runs agx_hp1_articulated_step_joint_force (with the IMU input and the effort DOFs above, if any), which
+        writes them from the last sub-step: row i >= 1 of joint_wrench is the force and the torque (about the joint origin) body i's
+        parent exerts on it through joint i, both in body i's frame, row 0 is zero; dof_force is each joint's torque along its axis."""
         self.lib = _lib.load()
         self.device = torch.device(device)
         if self.device.type != "cuda":
@@ -334,6 +338,7 @@ class Hp1Engine:
         self._init_body_state()
         self._init_imu(imu_body)
         self._init_effort()
+        self._init_joint_force(joint_force)
         z = lambda *s, dt=torch.float32: torch.zeros(*s, dtype=dt, device=dev)
         self.root_state = z(N, 13)
         self.root_state[:, 6] = 1.0
@@ -443,6 +448,18 @@ class Hp1Engine:
         self._effort = self.articulation.effort_struct()
         self._effort.effort = self.dof_actuation_force.data_ptr()
         self._effort_ref = C.byref(self._effort)
+
+    def _init_joint_force(self, joint_force):
+        """joint_wrench [N,B,6] and dof_force [N,D] of an articulated robot with joint_force (None otherwise), zero until the first step"""
+        self.joint_wrench, self.dof_force = None, None
+        if not joint_force:
+            return
+        if self.articulation is None:
+            raise ValueError("joint_force belongs to an articulated robot (Hp1Engine(articulation=...)): a rigid robot has no joints to "
+                             "sense")
+        B, D = self.articulation.bodies.num_bodies, self.articulation.num_dofs
+        self.joint_wrench = torch.zeros(self.N, B, 6, dtype=torch.float32, device=self.device)
+        self.dof_force = torch.zeros(self.N, D, dtype=torch.float32, device=self.device)
 
     def _host_tensor(self, shape, dtype):
         nbytes = max(1, int(np.prod(shape))) * torch.empty((), dtype=dtype).element_size()
@@ -576,6 +593,13 @@ class Hp1Engine:
         self._buf.dist_offset = dist_offset
         if physics_steps is not None:
             self.cfg.physics_steps = int(physics_steps)
+        if self.joint_wrench is not None:
+            imu = self.imu_input is not None
+            _lib.check(self.lib.agx_hp1_articulated_step_joint_force(
+                self._cfg_ref, self._buf_ref, self._art_ref, self._effort_ref if self._effort is not None else None,
+                self.imu_body if imu else 0, self._ptr(self.imu_input), self.joint_wrench.data_ptr(), self.dof_force.data_ptr(),
+                self._stream()), "agx_hp1_articulated_step_joint_force")
+            return
         if self._effort is not None:
             imu = self.imu_input is not None
             _lib.check(self.lib.agx_hp1_articulated_step_effort(self._cfg_ref, self._buf_ref, self._art_ref, self._effort_ref,

@@ -301,6 +301,23 @@ typedef struct AgxJointEffort {
 int agx_hp1_articulated_step_effort(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, const AgxArticulation* art,
                                     const AgxJointEffort* effort, int imu_body, float* imu_input, void* stream);
 
+/* Joint force sensing: agx_hp1_articulated_step_effort (effort != NULL) or agx_hp1_articulated_step (effort == NULL), with the IMU
+ * input where imu_input != NULL (imu_body as in agx_hp1_articulated_step_imu), and on the LAST sub-step of the launch, at that
+ * sub-step's start state and with its accelerations:
+ *   joint_wrench [N,B,6] out, bodies in table order: row i >= 1 is the wrench body i's parent exerts on body i through joint i --
+ *     the force (3), then the torque about the joint origin (3), both in body i's frame; it includes the drive, effort and passive
+ *     damping torque along the axis and the constraint reaction in the five other directions, not a limit force (the limit is a
+ *     projection, not a constraint).  Row 0 is zero.
+ *   dof_force [N,D] out: DOF i - 1 = axis_i . (row i's torque), the joint torque at the unprojected end-of-step state
+ *     (k (q* - q') + d (q-dot* - q-dot') for a position DOF, tau_e - d q-dot' for an effort DOF; q-dot' = q-dot + dt q-ddot,
+ *     q' = q + dt q-dot').
+ * With physics_steps = 0 both are zero.  Both dense and 16-byte aligned; dof_force may be NULL for a one-body tree.  The state is
+ * computed by the same source as the other articulated steps; a separate kernel, so the device's multiply-add contraction may round
+ * it differently (float32 rounding).  Capturable: no allocation, no synchronisation. */
+int agx_hp1_articulated_step_joint_force(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, const AgxArticulation* art,
+                                         const AgxJointEffort* effort, int imu_body, float* imu_input, float* joint_wrench,
+                                         float* dof_force, void* stream);
+
 /* Pose and velocity of every body of an articulated robot, from the root state and art->dof_state (the other [N,...] arrays of
  * `art` are not read).  root_state [N,stride] (stride >= 13, rows as AgxHp1Buffers.root_state); body_state [N,B,13] out, dense,
  * 16-byte aligned, bodies in table order, each row laid out like a root_state row:
