@@ -1,9 +1,12 @@
-// Robot-environment contact (DESIGN.md "Contact mode"): the robot's collision sphere against the scene objects and the ground
-// plane, one velocity-level sequential-impulse solve after each physics sub-step.  This header holds the solve: a contact list in,
-// the velocity change and the total impulse out.  The contact search (BVH descent, closest point) is in hp2_raycast.cu.
-// AGX_DEV: device-only in the product (hp2_raycast.cu, compiled with -fmad=false), host+device in the CPU shadow build
-// (tests/csrc/contact_shadow.cu, -ffp-contract=off).  oracle/contact_oracle.py restates every line in numpy float32 in the same
-// operation order, so the three agree bit for bit.
+// Contact (DESIGN.md "Contact mode"): one velocity-level sequential-impulse solve after each physics sub-step, for the robot's
+// collision sphere against the scene objects and the ground plane (contact_env), for free obstacles against the ground plane
+// (obstacle_ground_row) and for free obstacles against each other (obstacle_contacts_solve).  Every contact has two sides: side A
+// takes the impulse +dP and side O takes -dP.  One per-contact step (contact_step) runs the normal row and the friction row of all
+// of them; the side types say where each side's point velocity comes from, whether it adds to the inverse effective mass and
+// whether it takes the impulse.  The robot's contact search (BVH descent, closest point) is in hp2_raycast.cu.
+// AGX_DEV: device-only in the product (hp2_raycast.cu and obstacles.cu, compiled with -fmad=false), host+device in the CPU shadow
+// build (tests/csrc/contact_shadow.cu, -ffp-contract=off).  oracle/contact*_oracle.py restate every solve in numpy float32 in the
+// same operation order, so the three agree bit for bit.
 #pragma once
 #include "../../include/aerial_gym_b200.h"
 #include "agx_math.cuh"
@@ -70,121 +73,7 @@ AGX_DEV void obstacle_point_vel(const float* row, const float* p, float* u) {
     cvel(row + 7, row + 10, r, u);
 }
 
-// One env: n contacts of the sphere whose centre is pos and orientation q (x, y, z, w).  v, w: world linear / angular velocity,
-// updated in place.  imp: sum of the accumulated contact impulses (world frame).
-// MOVING (agx_hp2_contact_moving): u[i] is the velocity of contact i's obstacle at its contact point, and both rows act on the
-// relative velocity v_robot(p) - u.  The obstacle is kinematic (infinite mass), so only the robot's velocity changes.  Without
-// MOVING no u is read and the code is the static solve's.
-template <bool MOVING = false>
-AGX_DEV void contact_solve(const AgxContactParams& P, const float* pos, const float* q, float* v, float* w, const ContactPt* c, int n,
-                           float* imp, const float (*u)[3] = nullptr) {
-    const float x = q[0], y = q[1], z = q[2], qw = q[3];
-    float R[9];
-    R[0] = 1.0f - 2.0f * (y * y + z * z);
-    R[1] = 2.0f * (x * y - z * qw);
-    R[2] = 2.0f * (x * z + y * qw);
-    R[3] = 2.0f * (x * y + z * qw);
-    R[4] = 1.0f - 2.0f * (x * x + z * z);
-    R[5] = 2.0f * (y * z - x * qw);
-    R[6] = 2.0f * (x * z - y * qw);
-    R[7] = 2.0f * (y * z + x * qw);
-    R[8] = 1.0f - 2.0f * (x * x + y * y);
-    float com[3], A[9], Iw[9];
-    cmatvec(R, P.com, com);
-    for (int i = 0; i < 3; ++i) com[i] = pos[i] + com[i];
-    for (int i = 0; i < 3; ++i)  // A = R I^-1, Iw = A R^T
-        for (int j = 0; j < 3; ++j) A[3 * i + j] = R[3 * i] * P.inertia_inv[j] + R[3 * i + 1] * P.inertia_inv[3 + j] + R[3 * i + 2] * P.inertia_inv[6 + j];
-    for (int i = 0; i < 3; ++i)
-        for (int j = 0; j < 3; ++j) Iw[3 * i + j] = A[3 * i] * R[3 * j] + A[3 * i + 1] * R[3 * j + 1] + A[3 * i + 2] * R[3 * j + 2];
-    const float inv_m = 1.0f / P.mass;
-    float r[AGX_CONTACT_MAX][3], kn[AGX_CONTACT_MAX], bias[AGX_CONTACT_MAX], ln[AGX_CONTACT_MAX], lt[AGX_CONTACT_MAX][3];
-    for (int i = 0; i < n; ++i) {
-        for (int k = 0; k < 3; ++k) {
-            r[i][k] = c[i].p[k] - com[k];
-            lt[i][k] = 0.0f;
-        }
-        kn[i] = ckeff(r[i], c[i].n, inv_m, Iw);
-        bias[i] = fminf(fmaxf(c[i].depth - P.rest_offset, 0.0f) / P.dt, P.max_depenetration_velocity);
-        ln[i] = 0.0f;
-    }
-    for (int it = 0; it < P.iterations; ++it) {
-        for (int i = 0; i < n; ++i) {
-            const float* nn = c[i].n;
-            float vr[3], dP[3];
-            // normal: accumulated impulse >= 0, target separating velocity bias
-            cvel(v, w, r[i], vr);
-            if (MOVING)
-                for (int k = 0; k < 3; ++k) vr[k] = vr[k] - u[i][k];
-            float dl = (bias[i] - cdot(nn, vr)) / kn[i];
-            const float l1 = fmaxf(ln[i] + dl, 0.0f);
-            dl = l1 - ln[i];
-            ln[i] = l1;
-            for (int k = 0; k < 3; ++k) dP[k] = nn[k] * dl;
-            capply(dP, r[i], inv_m, Iw, v, w);
-            // friction: drive the tangential velocity to 0, accumulated impulse inside the circle mu * ln
-            cvel(v, w, r[i], vr);
-            if (MOVING)
-                for (int k = 0; k < 3; ++k) vr[k] = vr[k] - u[i][k];
-            const float vn = cdot(nn, vr);
-            float vt[3], l2[3];
-            for (int k = 0; k < 3; ++k) {
-                vt[k] = vr[k] - nn[k] * vn;
-                l2[k] = lt[i][k];
-            }
-            const float s = sqrtf(cdot(vt, vt));
-            if (s > 0.0f) {
-                float t[3];
-                for (int k = 0; k < 3; ++k) t[k] = vt[k] / s;
-                const float dt_ = s / ckeff(r[i], t, inv_m, Iw);
-                for (int k = 0; k < 3; ++k) l2[k] = l2[k] - t[k] * dt_;
-            }
-            const float mag = sqrtf(cdot(l2, l2)), lim = P.friction * ln[i];
-            if (mag > lim) {
-                const float f = lim / mag;
-                for (int k = 0; k < 3; ++k) l2[k] = l2[k] * f;
-            }
-            for (int k = 0; k < 3; ++k) {
-                dP[k] = l2[k] - lt[i][k];
-                lt[i][k] = l2[k];
-            }
-            capply(dP, r[i], inv_m, Iw, v, w);
-        }
-    }
-    imp[0] = imp[1] = imp[2] = 0.0f;
-    for (int i = 0; i < n; ++i)
-        for (int k = 0; k < 3; ++k) imp[k] = imp[k] + c[i].n[k] * ln[i] + lt[i][k];
-}
-
-// the per-env epilogue: solve, contact force = impulse / dt, crash flag when |F| exceeds the threshold (the reference's rule)
-template <bool MOVING = false>
-AGX_DEV void contact_env(const AgxContactParams& P, float* rs, const ContactPt* c, int n, float* force, uint8_t* crash,
-                         const float (*u)[3] = nullptr) {
-    float v[3] = {rs[7], rs[8], rs[9]}, w[3] = {rs[10], rs[11], rs[12]}, imp[3];
-    contact_solve<MOVING>(P, rs, rs + 3, v, w, c, n, imp, u);
-    for (int k = 0; k < 3; ++k) {
-        rs[7 + k] = v[k];
-        rs[10 + k] = w[k];
-        force[k] = imp[k] / P.dt;
-    }
-    if (sqrtf(cdot(force, force)) > P.force_threshold) *crash = 1;
-}
-
-// ---- Dynamic obstacles (agx_hp2_contact_dynamic): each obstacle asset is a free rigid body of finite mass, and every contact
-// impulse acts on the robot and on that body.  Separate functions, so that the static and moving instantiations above keep their
-// machine code.
-
-// One obstacle asset in the two-body solve.  Its twist is kept in the asset row's form: v is the velocity of the asset's origin x
-// (not of its COM c), w the angular velocity, both world frame.
-struct ContactBody {
-    float x[3], q[4], v[3], w[3];  // the asset row: origin, orientation (x, y, z, w), twist (updated by the solve)
-    float c[3];                    // COM, world
-    float oc[3];                   // x - c
-    float inv_m;
-    float Iw[9];                   // world inverse inertia R I^-1 R^T
-    bool free;                     // inv_m > 0 or a non-zero inverse inertia; otherwise kinematic: the solve reads its twist only
-};
-
-// R (row-major) of the unit quaternion q (x, y, z, w): contact_solve's expressions
+// R (row-major) of the unit quaternion q (x, y, z, w)
 AGX_DEV void cquat_R(const float* q, float* R) {
     const float x = q[0], y = q[1], z = q[2], qw = q[3];
     R[0] = 1.0f - 2.0f * (y * y + z * z);
@@ -198,7 +87,7 @@ AGX_DEV void cquat_R(const float* q, float* R) {
     R[8] = 1.0f - 2.0f * (x * x + y * y);
 }
 
-// world inverse inertia R I^-1 R^T, in contact_solve's order (A = R I^-1, Iw = A R^T)
+// world inverse inertia R I^-1 R^T (A = R I^-1, Iw = A R^T)
 AGX_DEV void cworld_inv_inertia(const float* R, const float* ii, float* Iw) {
     float A[9];
     for (int i = 0; i < 3; ++i)
@@ -206,6 +95,20 @@ AGX_DEV void cworld_inv_inertia(const float* R, const float* ii, float* Iw) {
     for (int i = 0; i < 3; ++i)
         for (int j = 0; j < 3; ++j) Iw[3 * i + j] = A[3 * i] * R[3 * j] + A[3 * i + 1] * R[3 * j + 1] + A[3 * i + 2] * R[3 * j + 2];
 }
+
+// ---- Obstacle assets as bodies of finite mass (agx_hp2_contact_dynamic, agx_obstacle_ground_contact,
+// agx_obstacle_obstacle_contact).
+
+// One obstacle asset in a solve.  Its twist is kept in the asset row's form: v is the velocity of the asset's origin x (not of its
+// COM c), w the angular velocity, both world frame.
+struct ContactBody {
+    float x[3], q[4], v[3], w[3];  // the asset row: origin, orientation (x, y, z, w), twist (updated by the solve)
+    float c[3];                    // COM, world
+    float oc[3];                   // x - c
+    float inv_m;
+    float Iw[9];                   // world inverse inertia R I^-1 R^T
+    bool free;                     // inv_m > 0 or a non-zero inverse inertia; otherwise kinematic: the solve reads its twist only
+};
 
 // the body of an asset row (x y z qx qy qz qw vx vy vz wx wy wz) and its mass-table entry
 AGX_DEV void contact_body_load(ContactBody& b, const float* row, const AgxObstacleMass& m) {
@@ -265,96 +168,6 @@ AGX_DEV void cbody_apply(const float* P, const float* s, ContactBody& b) {
     }
 }
 
-// contact_solve with two bodies per contact: body[i] is the index in B of contact i's obstacle, -1 for the ground (at rest,
-// infinite mass).  The relative velocity is v_robot(p) - (v_a + w_a x (p - x_a)); the inverse effective mass along d adds the
-// body's 1/m_a + (s x d) . I_a,w^-1 (s x d) with s = p - c_a; each impulse dP goes +dP to the robot and -dP to the body.  Contacts
-// on one body see each other's updates within a pass.  With every body kinematic the arithmetic is contact_solve<true>'s.
-AGX_DEV void contact_solve_dynamic(const AgxContactParams& P, const float* pos, const float* q, float* v, float* w, const ContactPt* c,
-                                   int n, float* imp, const int* body, ContactBody* B) {
-    float R[9], com[3], Iw[9];
-    cquat_R(q, R);
-    cmatvec(R, P.com, com);
-    for (int i = 0; i < 3; ++i) com[i] = pos[i] + com[i];
-    cworld_inv_inertia(R, P.inertia_inv, Iw);
-    const float inv_m = 1.0f / P.mass;
-    float r[AGX_CONTACT_MAX][3], ra[AGX_CONTACT_MAX][3], sa[AGX_CONTACT_MAX][3];
-    float kn[AGX_CONTACT_MAX], bias[AGX_CONTACT_MAX], ln[AGX_CONTACT_MAX], lt[AGX_CONTACT_MAX][3];
-    for (int i = 0; i < n; ++i) {
-        const int b = body[i];
-        for (int k = 0; k < 3; ++k) {
-            r[i][k] = c[i].p[k] - com[k];
-            ra[i][k] = b >= 0 ? c[i].p[k] - B[b].x[k] : 0.0f;
-            sa[i][k] = b >= 0 ? c[i].p[k] - B[b].c[k] : 0.0f;
-            lt[i][k] = 0.0f;
-        }
-        kn[i] = ckeff(r[i], c[i].n, inv_m, Iw);
-        if (b >= 0) kn[i] = kn[i] + ckeff(sa[i], c[i].n, B[b].inv_m, B[b].Iw);
-        bias[i] = fminf(fmaxf(c[i].depth - P.rest_offset, 0.0f) / P.dt, P.max_depenetration_velocity);
-        ln[i] = 0.0f;
-    }
-    for (int it = 0; it < P.iterations; ++it) {
-        for (int i = 0; i < n; ++i) {
-            const float* nn = c[i].n;
-            const int b = body[i];
-            float vr[3], u[3], dP[3], nP[3];
-            // normal: accumulated impulse >= 0, target separating velocity bias
-            cvel(v, w, r[i], vr);
-            if (b >= 0) {
-                cvel(B[b].v, B[b].w, ra[i], u);
-                for (int k = 0; k < 3; ++k) vr[k] = vr[k] - u[k];
-            }
-            float dl = (bias[i] - cdot(nn, vr)) / kn[i];
-            const float l1 = fmaxf(ln[i] + dl, 0.0f);
-            dl = l1 - ln[i];
-            ln[i] = l1;
-            for (int k = 0; k < 3; ++k) dP[k] = nn[k] * dl;
-            capply(dP, r[i], inv_m, Iw, v, w);
-            if (b >= 0 && B[b].free) {
-                for (int k = 0; k < 3; ++k) nP[k] = -dP[k];
-                cbody_apply(nP, sa[i], B[b]);
-            }
-            // friction: drive the tangential relative velocity to 0, accumulated impulse inside the circle mu * ln
-            cvel(v, w, r[i], vr);
-            if (b >= 0) {
-                cvel(B[b].v, B[b].w, ra[i], u);
-                for (int k = 0; k < 3; ++k) vr[k] = vr[k] - u[k];
-            }
-            const float vn = cdot(nn, vr);
-            float vt[3], l2[3];
-            for (int k = 0; k < 3; ++k) {
-                vt[k] = vr[k] - nn[k] * vn;
-                l2[k] = lt[i][k];
-            }
-            const float s = sqrtf(cdot(vt, vt));
-            if (s > 0.0f) {
-                float t[3];
-                for (int k = 0; k < 3; ++k) t[k] = vt[k] / s;
-                float kt = ckeff(r[i], t, inv_m, Iw);
-                if (b >= 0) kt = kt + ckeff(sa[i], t, B[b].inv_m, B[b].Iw);
-                const float dt_ = s / kt;
-                for (int k = 0; k < 3; ++k) l2[k] = l2[k] - t[k] * dt_;
-            }
-            const float mag = sqrtf(cdot(l2, l2)), lim = P.friction * ln[i];
-            if (mag > lim) {
-                const float f = lim / mag;
-                for (int k = 0; k < 3; ++k) l2[k] = l2[k] * f;
-            }
-            for (int k = 0; k < 3; ++k) {
-                dP[k] = l2[k] - lt[i][k];
-                lt[i][k] = l2[k];
-            }
-            capply(dP, r[i], inv_m, Iw, v, w);
-            if (b >= 0 && B[b].free) {
-                for (int k = 0; k < 3; ++k) nP[k] = -dP[k];
-                cbody_apply(nP, sa[i], B[b]);
-            }
-        }
-    }
-    imp[0] = imp[1] = imp[2] = 0.0f;
-    for (int i = 0; i < n; ++i)
-        for (int k = 0; k < 3; ++k) imp[k] = imp[k] + c[i].n[k] * ln[i] + lt[i][k];
-}
-
 // write a free body back to its asset row: the new twist, and the first-order position correction x += dt dv,
 // q = normalize(dq(dw dt) (x) q) with dq(a) = (a / 2, 1), dv / dw = the solve's change of the twist.  The rest of the sub-step
 // then moves the obstacle with its post-solve velocity.
@@ -378,28 +191,237 @@ AGX_DEV void contact_body_store(const ContactBody& b, float* row, float dt) {
     }
 }
 
-// contact_env for dynamic obstacles: the two-body solve, the robot's outputs as contact_env writes them, then every free body of
-// B[0..nb) written back to rows[b]
-AGX_DEV void contact_env_dynamic(const AgxContactParams& P, float* rs, const ContactPt* c, int n, float* force, uint8_t* crash,
-                                 const int* body, ContactBody* B, int nb, float* const* rows) {
+// ---- The per-contact step shared by every solve.  Side A takes +dP, side O takes -dP: the robot against an obstacle or the
+// ground, an asset against the ground, asset j against asset i.  The relative velocity is A's point velocity minus O's, the
+// inverse effective mass along d is A's term plus O's, and A takes its impulse before O.  An A side has vel / keff / apply; an O
+// side has sub_vel / add_keff / apply_neg, which skip a term the side does not have rather than add a zero, so that every solve
+// keeps the arithmetic (and the bits) of its oracle.
+
+// the robot, COM form: lever arm r = p - com
+struct RobotSide {
+    const float* r;
+    float inv_m;
+    const float* Iw;
+    float *v, *w;
+    AGX_DEV void vel(float* o) const { cvel(v, w, r, o); }
+    AGX_DEV float keff(const float* d) const { return ckeff(r, d, inv_m, Iw); }
+    AGX_DEV void apply(const float* P) const { capply(P, r, inv_m, Iw, v, w); }
+};
+
+// an asset body, origin form: its point velocity at lever arm r = p - x, its inverse effective mass and impulse at s = p - c.  A
+// kinematic body (not free) takes no impulse.
+struct BodySide {
+    ContactBody& b;
+    const float *r, *s;
+    AGX_DEV void vel(float* o) const { cvel(b.v, b.w, r, o); }
+    AGX_DEV float keff(const float* d) const { return ckeff(s, d, b.inv_m, b.Iw); }
+    AGX_DEV void apply(const float* P) const {
+        if (b.free) cbody_apply(P, s, b);
+    }
+    AGX_DEV void sub_vel(float* vr) const {
+        float u[3];
+        vel(u);
+        for (int k = 0; k < 3; ++k) vr[k] = vr[k] - u[k];
+    }
+    AGX_DEV float add_keff(float k, const float* d) const { return k + keff(d); }
+    AGX_DEV void apply_neg(const float* dP) const {
+        float nP[3];
+        for (int k = 0; k < 3; ++k) nP[k] = -dP[k];
+        apply(nP);
+    }
+};
+
+// a kinematic obstacle (infinite mass) whose velocity at the contact point is u
+struct PointVelSide {
+    const float* u;
+    AGX_DEV void sub_vel(float* vr) const {
+        for (int k = 0; k < 3; ++k) vr[k] = vr[k] - u[k];
+    }
+    AGX_DEV float add_keff(float k, const float*) const { return k; }
+    AGX_DEV void apply_neg(const float*) const {}
+};
+
+// a static obstacle or the ground: at rest, infinite mass
+struct RestSide {
+    AGX_DEV void sub_vel(float*) const {}
+    AGX_DEV float add_keff(float k, const float*) const { return k; }
+    AGX_DEV void apply_neg(const float*) const {}
+};
+
+// the dynamic robot solve's O side: the contact's asset body *b, or the ground at rest where b is null
+struct BodyOrRestSide {
+    ContactBody* b;
+    const float *r, *s;
+    AGX_DEV void sub_vel(float* vr) const {
+        if (b) BodySide{*b, r, s}.sub_vel(vr);
+    }
+    AGX_DEV float add_keff(float k, const float* d) const { return b ? BodySide{*b, r, s}.add_keff(k, d) : k; }
+    AGX_DEV void apply_neg(const float* dP) const {
+        if (b) BodySide{*b, r, s}.apply_neg(dP);
+    }
+};
+
+// one contact's solve state before the first pass: kn = the inverse effective mass along the normal, bias = the target separating
+// velocity, no accumulated impulse (ln, lt)
+template <class SA, class SO>
+AGX_DEV void contact_init(const AgxContactParams& P, const ContactPt& c, const SA& a, const SO& o, float& kn, float& bias, float& ln,
+                          float* lt) {
+    for (int k = 0; k < 3; ++k) lt[k] = 0.0f;
+    kn = o.add_keff(a.keff(c.n), c.n);
+    bias = fminf(fmaxf(c.depth - P.rest_offset, 0.0f) / P.dt, P.max_depenetration_velocity);
+    ln = 0.0f;
+}
+
+// one contact of one pass: the normal row, then the friction row.  nn: the contact normal (towards A); ln, lt: the accumulated
+// normal and friction impulses, updated.
+template <class SA, class SO>
+AGX_DEV void contact_step(const AgxContactParams& P, const float* nn, float kn, float bias, float& ln, float* lt, const SA& a,
+                          const SO& o) {
+    float vr[3], dP[3];
+    // normal: accumulated impulse >= 0, target separating velocity bias
+    a.vel(vr);
+    o.sub_vel(vr);
+    float dl = (bias - cdot(nn, vr)) / kn;
+    const float l1 = fmaxf(ln + dl, 0.0f);
+    dl = l1 - ln;
+    ln = l1;
+    for (int k = 0; k < 3; ++k) dP[k] = nn[k] * dl;
+    a.apply(dP);
+    o.apply_neg(dP);
+    // friction: drive the tangential relative velocity to 0, accumulated impulse inside the circle mu * ln
+    a.vel(vr);
+    o.sub_vel(vr);
+    const float vn = cdot(nn, vr);
+    float vt[3], l2[3];
+    for (int k = 0; k < 3; ++k) {
+        vt[k] = vr[k] - nn[k] * vn;
+        l2[k] = lt[k];
+    }
+    const float s = sqrtf(cdot(vt, vt));
+    if (s > 0.0f) {
+        float t[3];
+        for (int k = 0; k < 3; ++k) t[k] = vt[k] / s;
+        const float dt_ = s / o.add_keff(a.keff(t), t);
+        for (int k = 0; k < 3; ++k) l2[k] = l2[k] - t[k] * dt_;
+    }
+    const float mag = sqrtf(cdot(l2, l2)), lim = P.friction * ln;
+    if (mag > lim) {
+        const float f = lim / mag;
+        for (int k = 0; k < 3; ++k) l2[k] = l2[k] * f;
+    }
+    for (int k = 0; k < 3; ++k) {
+        dP[k] = l2[k] - lt[k];
+        lt[k] = l2[k];
+    }
+    a.apply(dP);
+    o.apply_neg(dP);
+}
+
+// ---- The robot's solve (agx_hp2_contact, agx_hp2_contact_moving, agx_hp2_contact_dynamic): the robot is side A of every contact.
+// The O sides come from a side set: init(i, c) precomputes what contact i's O side needs, side(i) is that side, finish(dt) runs
+// after the solve.
+
+// static obstacles and the ground
+struct RestSides {
+    AGX_DEV void init(int, const ContactPt&) {}
+    AGX_DEV RestSide side(int) const { return {}; }
+    AGX_DEV void finish(float) const {}
+};
+
+// moving obstacles: u[i] is the velocity of contact i's obstacle at its contact point (0 for the ground).  The obstacles are
+// kinematic, so only the robot's velocity changes; with u = 0 the arithmetic is the static solve's (x - 0 = x).
+struct PointVelSides {
+    const float (*u)[3];
+    AGX_DEV void init(int, const ContactPt&) {}
+    AGX_DEV PointVelSide side(int i) const { return {u[i]}; }
+    AGX_DEV void finish(float) const {}
+};
+
+// dynamic obstacles: body[i] is the index in B of contact i's obstacle, -1 for the ground (at rest, infinite mass); ra = p - x and
+// sa = p - c of each contact on its body.  Contacts on one body see each other's updates within a pass.  With every body kinematic
+// the arithmetic is the moving solve's.  Afterwards every free body of B[0..nb) is written back to rows[b].
+struct BodySides {
+    const int* body;
+    ContactBody* B;
+    int nb;
+    float* const* rows;
+    float ra[AGX_CONTACT_MAX][3], sa[AGX_CONTACT_MAX][3];
+    AGX_DEV BodySides(const int* body_, ContactBody* B_, int nb_, float* const* rows_) : body(body_), B(B_), nb(nb_), rows(rows_) {}
+    AGX_DEV void init(int i, const ContactPt& c) {
+        const int b = body[i];
+        for (int k = 0; k < 3; ++k) {
+            ra[i][k] = b >= 0 ? c.p[k] - B[b].x[k] : 0.0f;
+            sa[i][k] = b >= 0 ? c.p[k] - B[b].c[k] : 0.0f;
+        }
+    }
+    AGX_DEV BodyOrRestSide side(int i) { return {body[i] >= 0 ? B + body[i] : nullptr, ra[i], sa[i]}; }
+    AGX_DEV void finish(float dt) const {
+        for (int b = 0; b < nb; ++b)
+            if (B[b].free) contact_body_store(B[b], rows[b], dt);
+    }
+};
+
+// One env: n contacts of the sphere whose centre is pos and orientation q (x, y, z, w).  v, w: world linear / angular velocity,
+// updated in place.  imp: sum of the accumulated contact impulses on the robot (world frame).
+template <class O>
+AGX_DEV void contact_solve(const AgxContactParams& P, const float* pos, const float* q, float* v, float* w, const ContactPt* c, int n,
+                           float* imp, O& o) {
+    float R[9], com[3], Iw[9];
+    cquat_R(q, R);
+    cmatvec(R, P.com, com);
+    for (int i = 0; i < 3; ++i) com[i] = pos[i] + com[i];
+    cworld_inv_inertia(R, P.inertia_inv, Iw);
+    const float inv_m = 1.0f / P.mass;
+    float r[AGX_CONTACT_MAX][3], kn[AGX_CONTACT_MAX], bias[AGX_CONTACT_MAX], ln[AGX_CONTACT_MAX], lt[AGX_CONTACT_MAX][3];
+    for (int i = 0; i < n; ++i) {
+        for (int k = 0; k < 3; ++k) r[i][k] = c[i].p[k] - com[k];
+        o.init(i, c[i]);
+        contact_init(P, c[i], RobotSide{r[i], inv_m, Iw, v, w}, o.side(i), kn[i], bias[i], ln[i], lt[i]);
+    }
+    for (int it = 0; it < P.iterations; ++it)
+        for (int i = 0; i < n; ++i) contact_step(P, c[i].n, kn[i], bias[i], ln[i], lt[i], RobotSide{r[i], inv_m, Iw, v, w}, o.side(i));
+    imp[0] = imp[1] = imp[2] = 0.0f;
+    for (int i = 0; i < n; ++i)
+        for (int k = 0; k < 3; ++k) imp[k] = imp[k] + c[i].n[k] * ln[i] + lt[i][k];
+}
+
+// the per-env epilogue: solve, contact force = impulse / dt, crash flag when |F| exceeds the threshold (the reference's rule), then
+// the side set's finish (the dynamic solve's write-back)
+template <class O>
+AGX_DEV void contact_env_sides(const AgxContactParams& P, float* rs, const ContactPt* c, int n, float* force, uint8_t* crash, O o) {
     float v[3] = {rs[7], rs[8], rs[9]}, w[3] = {rs[10], rs[11], rs[12]}, imp[3];
-    contact_solve_dynamic(P, rs, rs + 3, v, w, c, n, imp, body, B);
+    contact_solve(P, rs, rs + 3, v, w, c, n, imp, o);
     for (int k = 0; k < 3; ++k) {
         rs[7 + k] = v[k];
         rs[10 + k] = w[k];
         force[k] = imp[k] / P.dt;
     }
     if (sqrtf(cdot(force, force)) > P.force_threshold) *crash = 1;
-    for (int b = 0; b < nb; ++b)
-        if (B[b].free) contact_body_store(B[b], rows[b], P.dt);
+    o.finish(P.dt);
+}
+
+// the epilogue of agx_hp2_contact (static obstacles and the ground) and, with MOVING, of agx_hp2_contact_moving (u: PointVelSides')
+template <bool MOVING = false>
+AGX_DEV void contact_env(const AgxContactParams& P, float* rs, const ContactPt* c, int n, float* force, uint8_t* crash,
+                         const float (*u)[3] = nullptr) {
+    if constexpr (MOVING)
+        contact_env_sides(P, rs, c, n, force, crash, PointVelSides{u});
+    else
+        contact_env_sides(P, rs, c, n, force, crash, RestSides{});
+}
+
+// the epilogue of agx_hp2_contact_dynamic (body, B, nb, rows: BodySides')
+AGX_DEV void contact_env_dynamic(const AgxContactParams& P, float* rs, const ContactPt* c, int n, float* force, uint8_t* crash,
+                                 const int* body, ContactBody* B, int nb, float* const* rows) {
+    contact_env_sides(P, rs, c, n, force, crash, BodySides(body, B, nb, rows));
 }
 
 // ---- Ground contact of free obstacles (agx_obstacle_ground_contact): one asset row against the plane z = 0 through the nv vertices
 // verts [nv,3] (asset frame) of its geometry, reach >= their largest distance from the asset origin.  Contacts: every vertex below
 // contact_offset, normal +z, depth -z, the AGX_CONTACT_MAX deepest kept (contact_insert on the key z: ties to the lower vertex index).
-// Solve: contact_solve_dynamic's per-contact step with the body alone against the ground at rest (infinite mass), then
-// contact_body_store.  Rows without a kept contact and kinematic rows are not written.  kept (may be NULL): the kept vertex
-// indices, deepest first.  Returns the number kept (0 for a row skipped by the reach test or kinematic).
+// Solve: the body as side A against the ground at rest (infinite mass), then contact_body_store.  Rows without a kept contact and
+// kinematic rows are not written.  kept (may be NULL): the kept vertex indices, deepest first.  Returns the number kept (0 for a row
+// skipped by the reach test or kinematic).
 AGX_DEV int obstacle_ground_row(const AgxContactParams& P, float* row, const AgxObstacleMass& m, const float* verts, int nv, float reach,
                                 int* kept) {
     if (row[2] - reach > P.contact_offset) return 0;
@@ -429,51 +451,11 @@ AGX_DEV int obstacle_ground_row(const AgxContactParams& P, float* row, const Agx
         for (int k = 0; k < 3; ++k) {
             ra[i][k] = c[i].p[k] - B.x[k];
             sa[i][k] = c[i].p[k] - B.c[k];
-            lt[i][k] = 0.0f;
         }
-        kn[i] = ckeff(sa[i], c[i].n, B.inv_m, B.Iw);
-        bias[i] = fminf(fmaxf(c[i].depth - P.rest_offset, 0.0f) / P.dt, P.max_depenetration_velocity);
-        ln[i] = 0.0f;
+        contact_init(P, c[i], BodySide{B, ra[i], sa[i]}, RestSide{}, kn[i], bias[i], ln[i], lt[i]);
     }
-    for (int it = 0; it < P.iterations; ++it) {
-        for (int i = 0; i < n; ++i) {
-            const float* nn = c[i].n;
-            float vr[3], dP[3];
-            // normal: accumulated impulse >= 0, target separating velocity bias
-            cvel(B.v, B.w, ra[i], vr);
-            float dl = (bias[i] - cdot(nn, vr)) / kn[i];
-            const float l1 = fmaxf(ln[i] + dl, 0.0f);
-            dl = l1 - ln[i];
-            ln[i] = l1;
-            for (int k = 0; k < 3; ++k) dP[k] = nn[k] * dl;
-            cbody_apply(dP, sa[i], B);
-            // friction: drive the tangential velocity at p to 0, accumulated impulse inside the circle mu * ln
-            cvel(B.v, B.w, ra[i], vr);
-            const float vn = cdot(nn, vr);
-            float vt[3], l2[3];
-            for (int k = 0; k < 3; ++k) {
-                vt[k] = vr[k] - nn[k] * vn;
-                l2[k] = lt[i][k];
-            }
-            const float s = sqrtf(cdot(vt, vt));
-            if (s > 0.0f) {
-                float t[3];
-                for (int k = 0; k < 3; ++k) t[k] = vt[k] / s;
-                const float dt_ = s / ckeff(sa[i], t, B.inv_m, B.Iw);
-                for (int k = 0; k < 3; ++k) l2[k] = l2[k] - t[k] * dt_;
-            }
-            const float mag = sqrtf(cdot(l2, l2)), lim = P.friction * ln[i];
-            if (mag > lim) {
-                const float f = lim / mag;
-                for (int k = 0; k < 3; ++k) l2[k] = l2[k] * f;
-            }
-            for (int k = 0; k < 3; ++k) {
-                dP[k] = l2[k] - lt[i][k];
-                lt[i][k] = l2[k];
-            }
-            cbody_apply(dP, sa[i], B);
-        }
-    }
+    for (int it = 0; it < P.iterations; ++it)
+        for (int i = 0; i < n; ++i) contact_step(P, c[i].n, kn[i], bias[i], ln[i], lt[i], BodySide{B, ra[i], sa[i]}, RestSide{});
     contact_body_store(B, row, P.dt);
     return n;
 }
@@ -687,84 +669,34 @@ struct ObstacleContact {
     float kn, bias, ln, lt[3];
 };
 
-// Sequential impulses over the env's contact list in order, `iterations` passes: obstacle_ground_row's per-contact step with body j
-// in the place of the body and body i in the place of the ground.  Relative velocity u_j(p) - u_i(p), u = v + w x (p - x); inverse
-// effective mass along d: the sum of both bodies' 1/m + (s x d) . I_w^-1 (s x d), s = p - c; impulse +dP to j, -dP to i.  A
-// kinematic body (not free) is read and never changed.  Every body of the list needs to be loaded in B.
+// the lever arms of contact o on body i (index 0) and body j (index 1): r = p - x, s = p - c
+AGX_DEV void obstacle_contact_arms(const ObstacleContact& o, const ContactBody* B, float (*r)[3], float (*s)[3]) {
+    for (int k = 0; k < 3; ++k) {
+        r[0][k] = o.c.p[k] - B[o.i].x[k];
+        r[1][k] = o.c.p[k] - B[o.j].x[k];
+        s[0][k] = o.c.p[k] - B[o.i].c[k];
+        s[1][k] = o.c.p[k] - B[o.j].c[k];
+    }
+}
+
+// Sequential impulses over the env's contact list in order, `iterations` passes: body j is side A, body i side O.  Relative
+// velocity u_j(p) - u_i(p), u = v + w x (p - x); inverse effective mass along d: the sum of both bodies' 1/m + (s x d) . I_w^-1 (s x d),
+// s = p - c; impulse +dP to j, -dP to i.  A kinematic body (not free) is read and never changed.  The lever arms are taken from B
+// on every pass.  Every body of the list needs to be loaded in B.
 AGX_DEV void obstacle_contacts_solve(const AgxContactParams& P, ContactBody* B, ObstacleContact* L, int n) {
     for (int q = 0; q < n; ++q) {
         ObstacleContact& o = L[q];
-        const ContactBody& bi = B[o.i];
-        const ContactBody& bj = B[o.j];
-        float si[3], sj[3];
-        for (int k = 0; k < 3; ++k) {
-            si[k] = o.c.p[k] - bi.c[k];
-            sj[k] = o.c.p[k] - bj.c[k];
-            o.lt[k] = 0.0f;
-        }
-        o.kn = ckeff(sj, o.c.n, bj.inv_m, bj.Iw) + ckeff(si, o.c.n, bi.inv_m, bi.Iw);
-        o.bias = fminf(fmaxf(o.c.depth - P.rest_offset, 0.0f) / P.dt, P.max_depenetration_velocity);
-        o.ln = 0.0f;
+        float r[2][3], s[2][3];
+        obstacle_contact_arms(o, B, r, s);
+        contact_init(P, o.c, BodySide{B[o.j], r[1], s[1]}, BodySide{B[o.i], r[0], s[0]}, o.kn, o.bias, o.ln, o.lt);
     }
-    for (int it = 0; it < P.iterations; ++it) {
+    for (int it = 0; it < P.iterations; ++it)
         for (int q = 0; q < n; ++q) {
             ObstacleContact& o = L[q];
-            ContactBody& bi = B[o.i];
-            ContactBody& bj = B[o.j];
-            const float* nn = o.c.n;
-            float ri[3], rj[3], si[3], sj[3];
-            for (int k = 0; k < 3; ++k) {
-                ri[k] = o.c.p[k] - bi.x[k];
-                rj[k] = o.c.p[k] - bj.x[k];
-                si[k] = o.c.p[k] - bi.c[k];
-                sj[k] = o.c.p[k] - bj.c[k];
-            }
-            float vr[3], u[3], dP[3], nP[3];
-            // normal: accumulated impulse >= 0, target separating velocity bias
-            cvel(bj.v, bj.w, rj, vr);
-            cvel(bi.v, bi.w, ri, u);
-            for (int k = 0; k < 3; ++k) vr[k] = vr[k] - u[k];
-            float dl = (o.bias - cdot(nn, vr)) / o.kn;
-            const float l1 = fmaxf(o.ln + dl, 0.0f);
-            dl = l1 - o.ln;
-            o.ln = l1;
-            for (int k = 0; k < 3; ++k) {
-                dP[k] = nn[k] * dl;
-                nP[k] = -dP[k];
-            }
-            if (bj.free) cbody_apply(dP, sj, bj);
-            if (bi.free) cbody_apply(nP, si, bi);
-            // friction: drive the tangential relative velocity at p to 0, accumulated impulse inside the circle mu * ln
-            cvel(bj.v, bj.w, rj, vr);
-            cvel(bi.v, bi.w, ri, u);
-            for (int k = 0; k < 3; ++k) vr[k] = vr[k] - u[k];
-            const float vn = cdot(nn, vr);
-            float vt[3], l2[3];
-            for (int k = 0; k < 3; ++k) {
-                vt[k] = vr[k] - nn[k] * vn;
-                l2[k] = o.lt[k];
-            }
-            const float s = sqrtf(cdot(vt, vt));
-            if (s > 0.0f) {
-                float t[3];
-                for (int k = 0; k < 3; ++k) t[k] = vt[k] / s;
-                const float dt_ = s / (ckeff(sj, t, bj.inv_m, bj.Iw) + ckeff(si, t, bi.inv_m, bi.Iw));
-                for (int k = 0; k < 3; ++k) l2[k] = l2[k] - t[k] * dt_;
-            }
-            const float mag = sqrtf(cdot(l2, l2)), lim = P.friction * o.ln;
-            if (mag > lim) {
-                const float f = lim / mag;
-                for (int k = 0; k < 3; ++k) l2[k] = l2[k] * f;
-            }
-            for (int k = 0; k < 3; ++k) {
-                dP[k] = l2[k] - o.lt[k];
-                o.lt[k] = l2[k];
-                nP[k] = -dP[k];
-            }
-            if (bj.free) cbody_apply(dP, sj, bj);
-            if (bi.free) cbody_apply(nP, si, bi);
+            float r[2][3], s[2][3];
+            obstacle_contact_arms(o, B, r, s);
+            contact_step(P, o.c.n, o.kn, o.bias, o.ln, o.lt, BodySide{B[o.j], r[1], s[1]}, BodySide{B[o.i], r[0], s[0]});
         }
-    }
 }
 
 }  // namespace agx

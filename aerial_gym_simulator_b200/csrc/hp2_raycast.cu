@@ -1001,90 +1001,8 @@ __device__ __noinline__ void mesh_closest(const AgxHp2Scene& sc, const MeshCtx& 
     }
 }
 
-// one thread per env: every object within reach (radius + contact_offset) gives its closest point, the ground plane one more;
-// the AGX_CONTACT_MAX nearest go to the solve.  sc.num_objects == 0: no scene.
-__global__ void __launch_bounds__(128)
-hp2_contact_kernel(const __grid_constant__ AgxHp2Scene sc, const __grid_constant__ AgxContactParams P, int num_envs,
-                   float* __restrict__ root_state, int stride, float* __restrict__ force, uint8_t* __restrict__ crashes,
-                   int32_t* __restrict__ contact_obj) {
-    const int e = blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= num_envs) return;
-    float* rs = root_state + (size_t)e * stride;
-    const v3 c{rs[0], rs[1], rs[2]};
-    const float reach = P.radius + P.contact_offset;
-    const float search = reach * reach;
-    agx::ContactPt cp[AGX_CONTACT_MAX];
-    float key[AGX_CONTACT_MAX];
-    int id[AGX_CONTACT_MAX];
-    int n = 0;
-    const int K = sc.num_objects;
-    if (K > 0) {
-        const int P2 = sc.leaves_pow2, L = sc.tris_per_object;
-        const float* nodes = sc.nodes + (size_t)e * (2 * P2 - 1) * kNodeFloats;
-        const int32_t* leaf = sc.leaf_object + (size_t)e * (P2 < 4 ? 4 : P2);
-        const float* tris = sc.tris + (size_t)e * K * L * kTriFloats;
-        int stack[24];
-        int sp = 0, node = 0;
-        while (true) {
-            const float* nd = nodes + (size_t)node * kNodeFloats;
-            float dx = fmaxf(fmaxf(nd[0] - c.x, c.x - nd[4]), 0.0f);
-            float dy = fmaxf(fmaxf(nd[1] - c.y, c.y - nd[5]), 0.0f);
-            float dz = fmaxf(fmaxf(nd[2] - c.z, c.z - nd[6]), 0.0f);
-            float box_d2 = dx * dx + dy * dy + dz * dz;
-            if (box_d2 <= search * 1.0001f + 1e-6f) {  // padded boxes + slack: culling only
-                if (node >= P2 - 1) {
-                    const int obj = leaf[node - (P2 - 1)];
-                    ObjClosest best{3.0e38f, v3{0.0f, 0.0f, 0.0f}, nullptr};
-                    if (obj >= 0 && sc.num_meshes && sc.obj_mesh_slot[((size_t)e * K + obj) * 2] >= 0) {
-                        mesh_closest(sc, mesh_ctx(sc, e), obj, c, search, best);
-                    } else if (obj >= 0) {
-                        const float4* tp = reinterpret_cast<const float4*>(tris + (size_t)obj * L * kTriFloats);
-                        for (int s = 0; s < L; ++s) {
-                            const float4 b = tp[3 * s + 1], cc = tp[3 * s + 2];
-                            if (b.x == 0.f && b.y == 0.f && b.z == 0.f && cc.x == 0.f && cc.y == 0.f && cc.z == 0.f) continue;  // padding
-                            tri_closest(c, tp + 3 * s, best);
-                        }
-                    }
-                    if (best.d2 <= search) {
-                        const float dist = sqrtf(best.d2);
-                        v3 nv;
-                        if (dist > 0.0f) {
-                            const v3 d = sub3(c, best.q);
-                            nv = v3{d.x / dist, d.y / dist, d.z / dist};
-                        } else {  // the centre lies on the surface: the triangle's face normal
-                            const float4 b = best.tri[1], cc = best.tri[2];
-                            nv = normalize3(cross3(v3{b.x, b.y, b.z}, v3{cc.x, cc.y, cc.z}));
-                        }
-                        const agx::ContactPt pt{{best.q.x, best.q.y, best.q.z}, {nv.x, nv.y, nv.z}, P.radius - dist};
-                        n = agx::contact_insert(cp, key, id, n, pt, dist, obj);
-                    }
-                } else {
-                    stack[sp++] = 2 * node + 2;
-                    node = 2 * node + 1;
-                    continue;
-                }
-            }
-            if (sp == 0) break;
-            node = stack[--sp];
-        }
-    }
-    if (P.ground_plane && c.z <= reach) {
-        const agx::ContactPt pt{{c.x, c.y, 0.0f}, {0.0f, 0.0f, 1.0f}, P.radius - c.z};
-        n = agx::contact_insert(cp, key, id, n, pt, c.z, K);
-    }
-    if (contact_obj)
-        for (int i = 0; i < AGX_CONTACT_MAX; ++i) contact_obj[(size_t)e * AGX_CONTACT_MAX + i] = i < n ? id[i] : -1;
-    float* f = force + (size_t)e * 3;
-    if (n == 0) {
-        f[0] = f[1] = f[2] = 0.0f;
-        return;
-    }
-    agx::contact_env(P, rs, cp, n, f, crashes + e);
-}
-
-// hp2_contact_kernel's contact search for one env (centre c), as a function: the nearest contacts in cp / key / id, their count
-// returned.  hp2_contact_kernel keeps its inline copy so that its machine code stays as it was verified: inlining this function
-// there lays out its stack frame differently.
+// the contact search for one env (centre c): every object within reach (radius + contact_offset) gives its closest point, the
+// ground plane one more; the AGX_CONTACT_MAX nearest in cp / key / id, their count returned.  sc.num_objects == 0: no scene.
 __device__ __forceinline__ int contact_search(const AgxHp2Scene& sc, const AgxContactParams& P, int e, v3 c, agx::ContactPt* cp, float* key,
                                               int* id) {
     const float reach = P.radius + P.contact_offset;
@@ -1146,6 +1064,28 @@ __device__ __forceinline__ int contact_search(const AgxHp2Scene& sc, const AgxCo
         n = agx::contact_insert(cp, key, id, n, pt, c.z, K);
     }
     return n;
+}
+
+// one thread per env: contact_search, then the solve of contact_core.cuh
+__global__ void __launch_bounds__(128)
+hp2_contact_kernel(const __grid_constant__ AgxHp2Scene sc, const __grid_constant__ AgxContactParams P, int num_envs,
+                   float* __restrict__ root_state, int stride, float* __restrict__ force, uint8_t* __restrict__ crashes,
+                   int32_t* __restrict__ contact_obj) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= num_envs) return;
+    float* rs = root_state + (size_t)e * stride;
+    agx::ContactPt cp[AGX_CONTACT_MAX];
+    float key[AGX_CONTACT_MAX];
+    int id[AGX_CONTACT_MAX];
+    const int n = contact_search(sc, P, e, v3{rs[0], rs[1], rs[2]}, cp, key, id);
+    if (contact_obj)
+        for (int i = 0; i < AGX_CONTACT_MAX; ++i) contact_obj[(size_t)e * AGX_CONTACT_MAX + i] = i < n ? id[i] : -1;
+    float* f = force + (size_t)e * 3;
+    if (n == 0) {
+        f[0] = f[1] = f[2] = 0.0f;
+        return;
+    }
+    agx::contact_env(P, rs, cp, n, f, crashes + e);
 }
 
 // hp2_contact_kernel with moving obstacles: each kept object contact also gets its obstacle's velocity at the contact point, from

@@ -1,4 +1,4 @@
-"""Build + load the CPU shadow of the contact solve (tests/csrc/contact_shadow.cu).  Test infrastructure only."""
+"""Build + load the CPU shadow of the contact solves (tests/csrc/contact_shadow.cu).  Test infrastructure only."""
 import ctypes as C
 import os
 import subprocess
@@ -31,10 +31,19 @@ def load():
     if _lib is None:
         from aerial_gym_simulator_b200 import _lib as A
         lib = C.CDLL(build())
-        lib.shadow_contact_solve.restype = None
-        lib.shadow_contact_solve.argtypes = [C.c_int, C.POINTER(A.AgxContactParams), C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
-                                             C.c_void_p, C.c_void_p]
-        lib.shadow_contact_select.restype = C.c_int
-        lib.shadow_contact_select.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        P, i, ll, v = C.POINTER(A.AgxContactParams), C.c_int, C.c_longlong, C.c_void_p
+        argtypes = {
+            "shadow_contact_solve": [i, P, v, i, v, v, v, v],
+            "shadow_contact_select": [i, v, v, v],
+            "shadow_contact_solve_moving": [i, P, v, i, v, v, v, v, v],
+            "shadow_obstacle_point_vel": [v, v, v],
+            "shadow_contact_solve_dynamic": [i, P, v, i, v, v, v, i, v, i, i, v, v, v, v],
+            "shadow_obstacle_ground": [ll, P, v, i, v, v, v, v, v, v, v],
+            "shadow_obstacle_obstacle": [i, i, P, v, i, v, v, v, v, v],
+        }
+        for name, args in argtypes.items():
+            f = getattr(lib, name)
+            f.argtypes = args
+            f.restype = C.c_int if name == "shadow_contact_select" else None
         _lib = lib
     return _lib

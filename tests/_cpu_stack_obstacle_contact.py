@@ -8,7 +8,7 @@ import ctypes as C
 
 import numpy as np
 
-from tests import _contact_ground_shadow, _contact_obstacle_shadow, _shadow
+from tests import _contact_shadow, _shadow
 
 _p = lambda a: C.c_void_p(a.ctypes.data)
 
@@ -21,8 +21,8 @@ def obstacle_obstacle_shadow(P, rows, mass, boxes, asset_box):
     count = np.zeros(E, np.int32)
     contacts = np.zeros((E, 128, 9), np.float32)
     keep = [np.ascontiguousarray(mass, np.float32), np.ascontiguousarray(boxes, np.float32), np.ascontiguousarray(asset_box, np.int32)]
-    _contact_obstacle_shadow.load().shadow_obstacle_obstacle(E, A, C.byref(P), _p(rows), stride, *(_p(x) for x in keep), _p(count),
-                                                             _p(contacts))
+    _contact_shadow.load().shadow_obstacle_obstacle(E, A, C.byref(P), _p(rows), stride, *(_p(x) for x in keep), _p(count),
+                                                    _p(contacts))
     return count, contacts
 
 
@@ -31,7 +31,7 @@ def ground_shadow(P, rows, mass, hull):
     E, A, stride = rows.shape
     keep = [mass, hull.vertices.numpy(), hull.file_offset.numpy(), hull.file_reach.numpy(), hull.asset_file.numpy(),
             np.zeros((E * A, 8), np.int32), np.zeros(E * A, np.int32)]
-    _contact_ground_shadow.load().shadow_obstacle_ground(E * A, C.byref(P), _p(rows), stride, *(_p(x) for x in keep))
+    _contact_shadow.load().shadow_obstacle_ground(E * A, C.byref(P), _p(rows), stride, *(_p(x) for x in keep))
 
 
 @contextlib.contextmanager

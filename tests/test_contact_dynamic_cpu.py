@@ -12,7 +12,7 @@ from aerial_gym_simulator_b200 import _lib
 from oracle import contact_dynamic_oracle as CD
 from oracle import contact_moving_oracle as CM
 from oracle import contact_oracle as CO
-from tests import _contact_dynamic_shadow
+from tests import _contact_shadow
 from tests.test_contact_cpu import params, random_contact_sets
 from tests.test_contact_moving_cpu import _full_params, shadow_moving
 
@@ -54,7 +54,7 @@ def shadow_dynamic(p, root, cts, count, ids, rows, obj_asset, mass):
     got, st = root.copy(), np.ascontiguousarray(rows, np.float32).copy()
     force = np.zeros((root.shape[0], 3), np.float32)
     crash = np.zeros(root.shape[0], np.uint8)
-    _contact_dynamic_shadow.load().shadow_contact_solve_dynamic(
+    _contact_shadow.load().shadow_contact_solve_dynamic(
         root.shape[0], C.byref(p), _p(got), 13, _p(cts), _p(count), _p(np.ascontiguousarray(ids, np.int32)), obj_asset.shape[1], _p(st),
         st.shape[1], 13, _p(np.ascontiguousarray(obj_asset, np.int32)), _p(np.ascontiguousarray(mass, np.float32)), _p(force), _p(crash))
     return got, force, crash.astype(bool), st

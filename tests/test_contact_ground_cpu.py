@@ -12,7 +12,7 @@ from aerial_gym_simulator_b200.env_manager.env_manager import _hull_vertices
 from aerial_gym_simulator_b200.hp2 import ObstacleHull, box_triangles, cylinder_triangles, icosphere_triangles
 from oracle import contact_dynamic_oracle as CD
 from oracle import contact_ground_oracle as CG
-from tests import _contact_ground_shadow
+from tests import _contact_shadow
 from tests.test_contact_cpu import params
 
 _p = lambda a: C.c_void_p(a.ctypes.data)
@@ -83,7 +83,7 @@ def shadow_ground(p, rows, mass, verts, off, reach, af):
     R = st.shape[0]
     kept = np.zeros((R, CMAX), np.int32)
     count = np.zeros(R, np.int32)
-    _contact_ground_shadow.load().shadow_obstacle_ground(
+    _contact_shadow.load().shadow_obstacle_ground(
         R, C.byref(p), _p(st), st.shape[1], _p(np.ascontiguousarray(mass, np.float32)), _p(np.ascontiguousarray(verts, np.float32)),
         _p(np.ascontiguousarray(off, np.int32)), _p(np.ascontiguousarray(reach, np.float32)), _p(np.ascontiguousarray(af, np.int32)),
         _p(kept), _p(count))

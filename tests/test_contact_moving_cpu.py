@@ -11,7 +11,7 @@ from aerial_gym_simulator_b200 import _lib
 from oracle import contact_moving_oracle as CM
 from oracle import contact_oracle as CO
 from oracle import hp2_oracle as RO
-from tests import _contact_moving_shadow, _contact_shadow
+from tests import _contact_shadow
 from tests.test_contact_cpu import _energy_never_rises, params, random_contact_sets
 
 _p = lambda a: C.c_void_p(a.ctypes.data)
@@ -37,8 +37,8 @@ def shadow_moving(p, root, cts, count, u):
     got = root.copy()
     force = np.zeros((root.shape[0], 3), np.float32)
     crash = np.zeros(root.shape[0], np.uint8)
-    _contact_moving_shadow.load().shadow_contact_solve_moving(root.shape[0], C.byref(p), _p(got), 13, _p(cts), _p(count),
-                                                              _p(np.ascontiguousarray(u, np.float32)), _p(force), _p(crash))
+    _contact_shadow.load().shadow_contact_solve_moving(root.shape[0], C.byref(p), _p(got), 13, _p(cts), _p(count),
+                                                       _p(np.ascontiguousarray(u, np.float32)), _p(force), _p(crash))
     return got, force, crash.astype(bool)
 
 
@@ -60,7 +60,7 @@ def test_shadow_moving_solve_matches_oracle_bit_for_bit(iterations, friction, se
     su = np.zeros(3, np.float32)
     for e in range(0, E, 7):
         for i in range(count[e]):
-            _contact_moving_shadow.load().shadow_obstacle_point_vel(_p(rows[e, i]), _p(np.ascontiguousarray(cts[e, i, 0:3])), _p(su))
+            _contact_shadow.load().shadow_obstacle_point_vel(_p(rows[e, i]), _p(np.ascontiguousarray(cts[e, i, 0:3])), _p(su))
             assert np.array_equal(su, u[e, i])
     assert np.abs(u[count > 0]).max() > 1.0
     p = _full_params(iterations=iterations, friction=friction)
