@@ -56,13 +56,6 @@ int validate_articulation(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, con
     return AGX_OK;
 }
 
-using ArtKernel = void (*)(const AgxHp1Config, const AgxHp1Buffers, const AgxArticulation);
-// per-body scratch sized for the tree: up to 9 bodies (a quadrotor with two joints per arm) or the full 16
-ArtKernel pick_art_kernel(int M, int B) {
-    if (M == 4) return B <= 9 ? articulated_step_kernel<4, 9> : articulated_step_kernel<4, AGX_ART_MAX_BODIES>;
-    return B <= 9 ? articulated_step_kernel<8, 9> : articulated_step_kernel<8, AGX_ART_MAX_BODIES>;
-}
-
 // ---- the step with the IMU input of one body (agx_hp1_articulated_step_imu): articulated_step_kernel plus one [9] store per env
 template <int M, int NB>
 __global__ void __launch_bounds__(kArtThreads)
@@ -71,12 +64,6 @@ articulated_step_imu_kernel(const __grid_constant__ AgxHp1Config cfg, const __gr
     const int env = blockIdx.x * blockDim.x + threadIdx.x;
     if (env >= cfg.num_envs) return;
     art_env_step<M, NB, true>(cfg, buf, art, env, imu_body, imu_input);
-}
-
-using ArtImuKernel = void (*)(const AgxHp1Config, const AgxHp1Buffers, const AgxArticulation, int, float*);
-ArtImuKernel pick_art_imu_kernel(int M, int B) {
-    if (M == 4) return B <= 9 ? articulated_step_imu_kernel<4, 9> : articulated_step_imu_kernel<4, AGX_ART_MAX_BODIES>;
-    return B <= 9 ? articulated_step_imu_kernel<8, 9> : articulated_step_imu_kernel<8, AGX_ART_MAX_BODIES>;
 }
 
 // ---- the step with effort-mode joints (agx_hp1_articulated_step_effort): one [D] read of the commanded torques per env and launch,
@@ -89,16 +76,6 @@ articulated_step_effort_kernel(const __grid_constant__ AgxHp1Config cfg, const _
     const int env = blockIdx.x * blockDim.x + threadIdx.x;
     if (env >= cfg.num_envs) return;
     art_env_step<M, NB, IMU, true>(cfg, buf, art, env, imu_body, imu_input, &eff);
-}
-
-using ArtEffortKernel = void (*)(const AgxHp1Config, const AgxHp1Buffers, const AgxArticulation, const AgxJointEffort, int, float*);
-template <bool IMU>
-ArtEffortKernel pick_art_effort_kernel_(int M, int B) {
-    if (M == 4) return B <= 9 ? articulated_step_effort_kernel<4, 9, IMU> : articulated_step_effort_kernel<4, AGX_ART_MAX_BODIES, IMU>;
-    return B <= 9 ? articulated_step_effort_kernel<8, 9, IMU> : articulated_step_effort_kernel<8, AGX_ART_MAX_BODIES, IMU>;
-}
-ArtEffortKernel pick_art_effort_kernel(int M, int B, bool imu) {
-    return imu ? pick_art_effort_kernel_<true>(M, B) : pick_art_effort_kernel_<false>(M, B);
 }
 
 // ---- the step with the joint forces (agx_hp1_articulated_step_joint_force): the effort kernel's arithmetic plus the rows of
@@ -152,13 +129,6 @@ articulated_step_joint_force_kernel(const __grid_constant__ AgxHp1Config cfg, co
     if (D) copy_warp_rows(dof_force + (size_t)env0 * D, s_warp, st, W, D, n, lane);
 }
 
-using ArtJointForceKernel = void (*)(const AgxHp1Config, const AgxHp1Buffers, const AgxArticulation, const AgxJointEffort, int, float*,
-                                     float*, float*);
-ArtJointForceKernel pick_art_joint_force_kernel(int M, int B) {
-    if (M == 4) return B <= 9 ? articulated_step_joint_force_kernel<4, 9> : articulated_step_joint_force_kernel<4, AGX_ART_MAX_BODIES>;
-    return B <= 9 ? articulated_step_joint_force_kernel<8, 9> : articulated_step_joint_force_kernel<8, AGX_ART_MAX_BODIES>;
-}
-
 // the checks of an effort table against art; its command array only where a DOF is in effort mode and there are envs
 int validate_effort(const AgxHp1Config* cfg, const AgxArticulation* art, const AgxJointEffort* effort) {
     bool any = false;
@@ -174,6 +144,20 @@ int validate_effort(const AgxHp1Config* cfg, const AgxArticulation* art, const A
         return agx_set_error(AGX_E_NULL, "effort->effort is NULL and a joint is in effort mode");
     return AGX_OK;
 }
+
+// the checks the step entries share: the articulation, the effort table where one is given, imu_body where the IMU is written
+int validate_step(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, const AgxArticulation* art, const AgxJointEffort* effort,
+                  bool imu, int imu_body) {
+    int rc = validate_articulation(cfg, buf, art);
+    if (rc) return rc;
+    if (effort && (rc = validate_effort(cfg, art, effort))) return rc;
+    if (imu && (imu_body < 0 || imu_body >= art->num_bodies))
+        return agx_set_error(AGX_E_INVALID, "imu_body must be in [0, %d) (got %d)", art->num_bodies, imu_body);
+    return AGX_OK;
+}
+
+// blocks of the step kernels: one env per thread
+int art_blocks(const AgxHp1Config* cfg) { return (cfg->num_envs + kArtThreads - 1) / kArtThreads; }
 
 // ---- per-body state (agx_hp1_articulated_body_state) ----------------------------------------------------------------------
 // One env per lane, one warp per block.  Each lane builds its env's B rows (13 B floats) in shared memory with art_body_states, the
@@ -244,70 +228,64 @@ extern "C" int agx_hp1_articulated_body_state(const AgxArticulation* art, int nu
     const int g = (num_envs + kBodyThreads - 1) / kBodyThreads;
     const int len = 13 * art->num_bodies;
     const size_t smem = sizeof(float) * kBodyThreads * (len + ((len & 1) ^ 1));  // <= 26.75 KB at 16 bodies
-    auto kern = art->num_bodies <= 9 ? articulated_body_state_kernel<9> : articulated_body_state_kernel<AGX_ART_MAX_BODIES>;
+    // the kernel has no motors: only the tree size of the instantiation applies
+    const auto kern = art_instantiation(4, art->num_bodies, [](auto, auto nb) { return articulated_body_state_kernel<nb>; });
     kern<<<g, kBodyThreads, smem, (cudaStream_t)stream>>>(*art, num_envs, root_state, root_state_stride, body_state);
     return agx_check_launch("articulated_body_state_kernel");
 }
 
 extern "C" int agx_hp1_articulated_step(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, const AgxArticulation* art, void* stream) {
-    int rc = validate_articulation(cfg, buf, art);
+    int rc = validate_step(cfg, buf, art, nullptr, false, 0);
     if (rc) return rc;
     if (cfg->num_envs == 0) return AGX_OK;
-    const int g = (cfg->num_envs + kArtThreads - 1) / kArtThreads;
-    pick_art_kernel(cfg->num_motors, art->num_bodies)<<<g, kArtThreads, 0, (cudaStream_t)stream>>>(*cfg, *buf, *art);
+    const auto kern = art_instantiation(cfg->num_motors, art->num_bodies, [](auto m, auto nb) { return articulated_step_kernel<m, nb>; });
+    kern<<<art_blocks(cfg), kArtThreads, 0, (cudaStream_t)stream>>>(*cfg, *buf, *art);
     return agx_check_launch("articulated_step_kernel");
 }
 
 extern "C" int agx_hp1_articulated_step_imu(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, const AgxArticulation* art, int imu_body,
                                             float* imu_input, void* stream) {
-    int rc = validate_articulation(cfg, buf, art);
+    int rc = validate_step(cfg, buf, art, nullptr, true, imu_body);
     if (rc) return rc;
-    if (imu_body < 0 || imu_body >= art->num_bodies)
-        return agx_set_error(AGX_E_INVALID, "imu_body must be in [0, %d) (got %d)", art->num_bodies, imu_body);
     if (!imu_input) return agx_set_error(AGX_E_NULL, "imu_input is NULL");
     if (cfg->num_envs == 0) return AGX_OK;
-    const int g = (cfg->num_envs + kArtThreads - 1) / kArtThreads;
-    pick_art_imu_kernel(cfg->num_motors, art->num_bodies)<<<g, kArtThreads, 0, (cudaStream_t)stream>>>(*cfg, *buf, *art, imu_body,
-                                                                                                      imu_input);
+    const auto kern =
+        art_instantiation(cfg->num_motors, art->num_bodies, [](auto m, auto nb) { return articulated_step_imu_kernel<m, nb>; });
+    kern<<<art_blocks(cfg), kArtThreads, 0, (cudaStream_t)stream>>>(*cfg, *buf, *art, imu_body, imu_input);
     return agx_check_launch("articulated_step_imu_kernel");
 }
 
 extern "C" int agx_hp1_articulated_step_effort(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, const AgxArticulation* art,
                                                const AgxJointEffort* effort, int imu_body, float* imu_input, void* stream) {
-    int rc = validate_articulation(cfg, buf, art);
+    int rc = validate_step(cfg, buf, art, effort, imu_input != nullptr, imu_body);
     if (rc) return rc;
     if (!effort) return agx_set_error(AGX_E_NULL, "effort is NULL");
-    if (imu_input && (imu_body < 0 || imu_body >= art->num_bodies))
-        return agx_set_error(AGX_E_INVALID, "imu_body must be in [0, %d) (got %d)", art->num_bodies, imu_body);
-    if ((rc = validate_effort(cfg, art, effort))) return rc;
     if (cfg->num_envs == 0) return AGX_OK;
-    const int g = (cfg->num_envs + kArtThreads - 1) / kArtThreads;
-    pick_art_effort_kernel(cfg->num_motors, art->num_bodies, imu_input != nullptr)<<<g, kArtThreads, 0, (cudaStream_t)stream>>>(
-        *cfg, *buf, *art, *effort, imu_body, imu_input);
+    const auto kern = art_instantiation(cfg->num_motors, art->num_bodies, [&](auto m, auto nb) {
+        return imu_input ? articulated_step_effort_kernel<m, nb, true> : articulated_step_effort_kernel<m, nb, false>;
+    });
+    kern<<<art_blocks(cfg), kArtThreads, 0, (cudaStream_t)stream>>>(*cfg, *buf, *art, *effort, imu_body, imu_input);
     return agx_check_launch("articulated_step_effort_kernel");
 }
 
 extern "C" int agx_hp1_articulated_step_joint_force(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, const AgxArticulation* art,
                                                     const AgxJointEffort* effort, int imu_body, float* imu_input, float* joint_wrench,
                                                     float* dof_force, void* stream) {
-    int rc = validate_articulation(cfg, buf, art);
+    int rc = validate_step(cfg, buf, art, effort, imu_input != nullptr, imu_body);
     if (rc) return rc;
-    if (effort && (rc = validate_effort(cfg, art, effort))) return rc;
-    if (imu_input && (imu_body < 0 || imu_body >= art->num_bodies))
-        return agx_set_error(AGX_E_INVALID, "imu_body must be in [0, %d) (got %d)", art->num_bodies, imu_body);
     if (cfg->num_envs == 0) return AGX_OK;
     if (!joint_wrench || (art->num_dofs > 0 && !dof_force)) return agx_set_error(AGX_E_NULL, "joint_wrench/dof_force is NULL");
     if (((uintptr_t)joint_wrench | (uintptr_t)dof_force) & 15)
         return agx_set_error(AGX_E_INVALID, "joint_wrench and dof_force must be 16-byte aligned");
     AgxJointEffort none = {};  // no effort DOF: every joint is stepped as agx_hp1_articulated_step steps it
-    const int g = (cfg->num_envs + kArtThreads - 1) / kArtThreads;
-    const ArtJointForceKernel kern = pick_art_joint_force_kernel(cfg->num_motors, art->num_bodies);
+    const auto kern =
+        art_instantiation(cfg->num_motors, art->num_bodies, [](auto m, auto nb) { return articulated_step_joint_force_kernel<m, nb>; });
     const size_t smem = sizeof(float) * kArtThreads * joint_force_row_stride(art->num_bodies);  // <= 56.8 KB at 16 bodies
     if (smem > 48 * 1024) {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return agx_set_error(AGX_E_CUDA, "cudaFuncSetAttribute: %s", cudaGetErrorString(e));
     }
-    kern<<<g, kArtThreads, smem, (cudaStream_t)stream>>>(*cfg, *buf, *art, effort ? *effort : none, imu_body, imu_input, joint_wrench,
-                                                          dof_force);
+    kern<<<art_blocks(cfg), kArtThreads, smem, (cudaStream_t)stream>>>(*cfg, *buf, *art, effort ? *effort : none, imu_body, imu_input,
+                                                                       joint_wrench, dof_force);
     return agx_check_launch("articulated_step_joint_force_kernel");
 }

@@ -10,12 +10,28 @@
 // "Rigid Body Dynamics Algorithms", 2008, section 7.3 with every X the identity), and the lever arms stay of the size of the robot
 // (~0.1 m), not of its distance from the world origin -- what keeps float32 usable.
 #pragma once
+#include <type_traits>
+
 #include "../../include/aerial_gym_b200.h"
 #include "agx_math.cuh"
 #include "disturbance_core.cuh"
 #include "hp1_core.cuh"
 
 namespace agx {
+
+// The instantiations of every articulated kernel, for its launcher in articulated.cu and for the CPU shadow alike: f(M, NB) with
+// std::integral_constant arguments, M = 4 or 8 motors and the per-body scratch sized for the tree -- up to 9 bodies (a quadrotor
+// with two joints per arm) or the full AGX_ART_MAX_BODIES.  Host code.
+template <class F>
+auto art_instantiation(int M, int B, F&& f) {
+    using M4 = std::integral_constant<int, 4>;
+    using M8 = std::integral_constant<int, 8>;
+    using NB9 = std::integral_constant<int, 9>;
+    using NBMax = std::integral_constant<int, AGX_ART_MAX_BODIES>;
+    const bool small = B <= 9;
+    if (M == 4) return small ? f(M4{}, NB9{}) : f(M4{}, NBMax{});
+    return small ? f(M8{}, NB9{}) : f(M8{}, NBMax{});
+}
 
 AGX_DEV M33 ld33(const float* a) {
     M33 r;
@@ -446,23 +462,11 @@ AGX_DEV void art_env_step(const AgxHp1Config& cfg, const AgxHp1Buffers& buf, con
             dtq = dtq + V3{d6[3], d6[4], d6[5]};
         }
         float a0[6];
-        if constexpr (JFORCE) {
-            const bool last = step + 1 == cfg.physics_steps;
-            float* imu = (last && imu_input) ? imu_input + (size_t)env * 9 : nullptr;
-            art_dynamics<NB, true, true, true>(art, s, q, qd, qs, qds, cfg.dt, grav, M, p.thrust, quat_rotate(s.q, df),
-                                               quat_rotate(s.q, dtq), a0, qdd, imu_body, imu, eff, last ? joint_wrench : nullptr,
-                                               dof_force);
-        } else if constexpr (EFFORT) {
-            float* imu = (IMU && step + 1 == cfg.physics_steps) ? imu_input + (size_t)env * 9 : nullptr;
-            art_dynamics<NB, IMU, true>(art, s, q, qd, qs, qds, cfg.dt, grav, M, p.thrust, quat_rotate(s.q, df), quat_rotate(s.q, dtq),
-                                        a0, qdd, imu_body, imu, eff);
-        } else if constexpr (IMU) {
-            float* imu = (step + 1 == cfg.physics_steps) ? imu_input + (size_t)env * 9 : nullptr;
-            art_dynamics<NB, true>(art, s, q, qd, qs, qds, cfg.dt, grav, M, p.thrust, quat_rotate(s.q, df), quat_rotate(s.q, dtq), a0,
-                                   qdd, imu_body, imu);
-        } else {
-            art_dynamics<NB>(art, s, q, qd, qs, qds, cfg.dt, grav, M, p.thrust, quat_rotate(s.q, df), quat_rotate(s.q, dtq), a0, qdd);
-        }
+        const bool last = step + 1 == cfg.physics_steps;
+        float* imu = (IMU && last && (!JFORCE || imu_input)) ? imu_input + (size_t)env * 9 : nullptr;
+        art_dynamics<NB, IMU, EFFORT, JFORCE>(art, s, q, qd, qs, qds, cfg.dt, grav, M, p.thrust, quat_rotate(s.q, df),
+                                              quat_rotate(s.q, dtq), a0, qdd, imu_body, imu, eff, (JFORCE && last) ? joint_wrench : nullptr,
+                                              dof_force);
         art_integrate(cfg, art, s, a0, q, qd, qdd);
     }
     if (cfg.physics_steps == 0) d = update_states(s);

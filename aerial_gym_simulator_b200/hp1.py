@@ -402,6 +402,22 @@ class Hp1Engine:
         self._plain = self.art is None  # no gather attached, no disturbance buffer or counter set: position_task_step's fast path
 
     # ---- plumbing ---------------------------------------------------------------------------
+    def _art_step_args(self):
+        """(name, arguments but the stream) of the articulated step entry physics_step runs for this robot, from the engine's state
+        at the call: with joint_force, the joint-force step (with the IMU input and the effort DOFs, if any); else with an effort
+        table, the effort step (with the IMU input, if any); else with imu_body, the IMU step; else the plain step"""
+        head = (self._cfg_ref, self._buf_ref, self._art_ref)
+        imu = (self.imu_body, self.imu_input.data_ptr()) if self.imu_input is not None else (0, None)
+        if self.joint_wrench is not None:
+            effort = self._effort_ref if self._effort is not None else None
+            out = (self.joint_wrench.data_ptr(), self.dof_force.data_ptr())
+            return "agx_hp1_articulated_step_joint_force", head + (effort,) + imu + out
+        if self._effort is not None:
+            return "agx_hp1_articulated_step_effort", head + (self._effort_ref,) + imu
+        if self.imu_input is not None:
+            return "agx_hp1_articulated_step_imu", head + imu
+        return "agx_hp1_articulated_step", head
+
     def _init_articulation(self, articulation, num_envs, debug_wrench, host_io):
         self.articulation, self.art = articulation, None
         self.dof_state = self.dof_position_setpoint = self.dof_velocity_setpoint = None
@@ -593,26 +609,9 @@ class Hp1Engine:
         self._buf.dist_offset = dist_offset
         if physics_steps is not None:
             self.cfg.physics_steps = int(physics_steps)
-        if self.joint_wrench is not None:
-            imu = self.imu_input is not None
-            _lib.check(self.lib.agx_hp1_articulated_step_joint_force(
-                self._cfg_ref, self._buf_ref, self._art_ref, self._effort_ref if self._effort is not None else None,
-                self.imu_body if imu else 0, self._ptr(self.imu_input), self.joint_wrench.data_ptr(), self.dof_force.data_ptr(),
-                self._stream()), "agx_hp1_articulated_step_joint_force")
-            return
-        if self._effort is not None:
-            imu = self.imu_input is not None
-            _lib.check(self.lib.agx_hp1_articulated_step_effort(self._cfg_ref, self._buf_ref, self._art_ref, self._effort_ref,
-                                                                self.imu_body if imu else 0, self._ptr(self.imu_input), self._stream()),
-                       "agx_hp1_articulated_step_effort")
-            return
-        if self.imu_input is not None:
-            _lib.check(self.lib.agx_hp1_articulated_step_imu(self._cfg_ref, self._buf_ref, self._art_ref, self.imu_body,
-                                                             self.imu_input.data_ptr(), self._stream()), "agx_hp1_articulated_step_imu")
-            return
         if self.art is not None:
-            _lib.check(self.lib.agx_hp1_articulated_step(self._cfg_ref, self._buf_ref, self._art_ref, self._stream()),
-                       "agx_hp1_articulated_step")
+            name, args = self._art_step_args()
+            _lib.check(getattr(self.lib, name)(*args, self._stream()), name)
             return
         _lib.check(self.lib.agx_hp1_physics_step(self._cfg_ref, self._buf_ref, self._stream()), "agx_hp1_physics_step")
 

@@ -1,12 +1,14 @@
 """CPU twin of an articulated robot's engine, on top of tests/_cpu_stack.py.  TEST INFRASTRUCTURE ONLY.
 
-``CpuArticulatedHp1Engine`` is ``CpuHp1Engine`` that also takes ``articulation=`` (an ArticulationSpec): the joint tensors and the
-AgxArticulation struct are set up by the PRODUCT's own ``Hp1Engine._init_articulation`` (on CPU tensors), and ``physics_step`` of
-an articulated robot runs the host shadow of articulated_core.cuh (tests/csrc/articulated_shadow.cu).  Without ``articulation`` it
-is ``CpuHp1Engine``.
+``CpuArticulatedHp1Engine`` is ``CpuHp1Engine`` that also takes ``articulation=`` (an ArticulationSpec), ``imu_body=`` and
+``joint_force=``: the joint tensors, body_state, imu_input, the effort table and joint_wrench / dof_force are set up by the PRODUCT's
+own ``Hp1Engine._init_*`` (on CPU tensors), and ``physics_step`` of an articulated robot runs the host shadow
+(tests/csrc/articulated_shadow.cu) of the entry the PRODUCT's ``Hp1Engine._art_step_args`` picks, with the same arguments:
+agx_hp1_articulated_step* -> shadow_art_step*.  ``update_body_state`` runs the shadow of agx_hp1_articulated_body_state.  Without
+``articulation`` it is ``CpuHp1Engine``.
 
 ``with articulated_cpu_stack():`` is ``cpu_stack()`` with EnvManager's engine swapped for this twin, so an EnvManager (and a task)
-with ``morphy_compliant`` runs end to end on the CPU.  ``articulated_twin_for_dryrun(module)`` does the same swap inside an already
+with an articulated robot runs end to end on the CPU.  ``articulated_twin_for_dryrun()`` does the same swap inside an already
 entered ``cpu_stack()`` -- what the ``--gpu-dryrun`` fixture of tests/conftest.py enters for a -m gpu test."""
 import contextlib
 import ctypes as C
@@ -19,9 +21,17 @@ from ._shadow_hp1 import ShadowHp1Engine
 
 
 class CpuArticulatedHp1Engine(CpuHp1Engine):
-    def __init__(self, spec, num_envs, device="cpu", *, articulation=None, debug_wrench=False, host_io=False, **kw):
+    _art_step_args = Hp1Engine._art_step_args
+
+    def __init__(self, spec, num_envs, device="cpu", *, articulation=None, imu_body=None, joint_force=False, debug_wrench=False,
+                 host_io=False, **kw):
         super().__init__(spec, num_envs, device, debug_wrench=debug_wrench, host_io=host_io, **kw)
         Hp1Engine._init_articulation(self, articulation, num_envs, debug_wrench, host_io)
+        Hp1Engine._init_body_state(self)
+        Hp1Engine._init_imu(self, imu_body)
+        Hp1Engine._init_effort(self)
+        Hp1Engine._init_joint_force(self, joint_force)
+        self._cfg_ref, self._buf_ref = C.byref(self.cfg), C.byref(self._buf)
 
     def position_task_step(self, actions, disturbance=None, physics_steps=None, mid_event=None):
         if self.art is not None:
@@ -33,7 +43,14 @@ class CpuArticulatedHp1Engine(CpuHp1Engine):
             ShadowHp1Engine.physics_step(self, actions.contiguous(), disturbance, physics_steps, dist_counter, dist_offset)
             return
         self._set_inputs(actions.contiguous(), disturbance, physics_steps, dist_counter, dist_offset)
-        assert _articulated_shadow.load().shadow_art_step(C.byref(self.cfg), C.byref(self._buf), C.byref(self.art)) == 0
+        name, args = self._art_step_args()
+        shadow = getattr(_articulated_shadow.load(), name.replace("agx_hp1_articulated_step", "shadow_art_step"))
+        assert shadow(*args) == 0
+
+    def update_body_state(self):
+        if self.art is None:
+            raise ValueError("body_state belongs to an articulated robot (Hp1Engine(articulation=...))")
+        _articulated_shadow.body_state(self.art, self.root_state, self.body_state)
 
 
 @contextlib.contextmanager

@@ -1,21 +1,17 @@
 """Per-body state of articulated robots on the CPU (DESIGN.md "Articulated robots"): art_body_states of articulated_core.cuh (host
-shadow, tests/csrc/articulated_body_state_shadow.cu) against oracle/articulated_body_state_oracle.py's float64 body_states(), the Global Tensor
+shadow, tests/csrc/articulated_shadow.cu) against oracle/articulated_body_state_oracle.py's float64 body_states(), the Global Tensor
 Dict keys and their refresh in EnvManager, ray-cast sensors on a link (cfg.parent_link), and the gimbal quadrotor's levelling."""
-import os
-import re
-import subprocess
-
 import numpy as np
 import pytest
 import torch
 
-from aerial_gym_simulator_b200 import _build
 from oracle import articulated_body_state_oracle as BO
 from oracle import articulated_oracle as AO
 from oracle import hp2_oracle as RO
 
-from . import _cpu_stack_body_state as BS
+from . import _articulated_shadow
 from . import _hp2_common as H2
+from ._cpu_stack_articulated import articulated_cpu_stack
 from .test_articulated_cpu import morphy_compliant, random_art, random_root, table_of
 
 EPS = float(np.finfo(np.float32).eps)
@@ -37,7 +33,7 @@ def _shadow_rows(art_spec, roots, dof):
     s.dof_state = dof_t.data_ptr()
     root_t = torch.tensor(np.asarray(roots, np.float32))
     out = torch.zeros(root_t.shape[0], s.num_bodies, 13)
-    BS.body_state(s, root_t, out)
+    _articulated_shadow.body_state(s, root_t, out)
     return out.numpy(), s, root_t.numpy()
 
 
@@ -137,19 +133,6 @@ def test_velocities_are_the_time_derivatives_of_the_forward_kinematics():
             assert np.abs(np.array([W[2, 1], W[0, 2], W[1, 0]]) - ref[i, 10:13]).max() < 1e-6
 
 
-def test_body_state_kernels_have_no_spills_and_no_stack():
-    """-Xptxas -v of articulated.cu: both instantiations of articulated_body_state_kernel are free of local memory"""
-    src = os.path.join(_build.CSRC, "articulated.cu")
-    r = subprocess.run([_build._nvcc()] + _build.NVCC_FLAGS + ["-Xptxas", "-v", "-c", src, "-o", os.devnull], capture_output=True,
-                       text=True)
-    assert r.returncode == 0, r.stderr
-    blocks = re.findall(r"Compiling entry function '(\S+)'.*?\n(.*?stack frame.*?)\n", r.stderr, re.S)
-    found = [(f, info) for f, info in blocks if "articulated_body_state_kernel" in f]
-    assert len(found) == 2, r.stderr
-    for f, info in found:
-        assert "0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads" in info, (f, info)
-
-
 # ---- EnvManager ---------------------------------------------------------------------------------------------------------------
 def _env(robot="morphy_compliant", env_name="empty_env", n=8, **args):
     from aerial_gym_simulator_b200.env_manager.env_manager import EnvManager
@@ -159,12 +142,12 @@ def _env(robot="morphy_compliant", env_name="empty_env", n=8, **args):
 def _expected_rows(env):
     eng = env.engine
     out = torch.zeros_like(eng.body_state)
-    BS.body_state(eng.art, eng.root_state, out)
+    _articulated_shadow.body_state(eng.art, eng.root_state, out)
     return out
 
 
 def test_gtd_keys_and_refresh_after_step_and_reset():
-    with BS.body_state_cpu_stack():
+    with articulated_cpu_stack():
         torch.manual_seed(0)
         env = _env(n=8)
         gtd = env.global_tensor_dict
@@ -191,7 +174,7 @@ def test_gtd_keys_and_refresh_after_step_and_reset():
 
 
 def test_rigid_robots_get_no_body_keys():
-    with BS.body_state_cpu_stack():
+    with articulated_cpu_stack():
         env = _env("base_quadrotor", n=4)
         assert "robot_body_state_tensor" not in env.global_tensor_dict and "robot_body_names" not in env.global_tensor_dict
         assert env.engine.body_state is None
@@ -228,7 +211,7 @@ def gimbal_camera_check(env, idx=None):
 
 
 def test_gimbal_camera_image_equals_oracle_at_the_link_pose():
-    with BS.body_state_cpu_stack():
+    with articulated_cpu_stack():
         torch.manual_seed(0)
         env = _env("base_quadrotor_with_gimbal_camera", "env_with_obstacles", n=4)
         assert env.sensor.robot_state.data_ptr() == env.engine.body_state[:, 2].data_ptr()
@@ -244,7 +227,7 @@ def test_gimbal_camera_image_equals_oracle_at_the_link_pose():
 
 
 def test_no_parent_link_reads_the_robot_state_and_the_mount():
-    with BS.body_state_cpu_stack():
+    with articulated_cpu_stack():
         torch.manual_seed(0)
         env = _env("base_quadrotor_with_camera", "env_with_obstacles", n=4)
         env.reset()
@@ -277,7 +260,7 @@ def _register_link_camera(name, link, base=None):
 
 def test_rigid_robot_camera_on_a_fixed_link_equals_a_base_camera_with_the_link_folded_in():
     _register_link_camera("_test_quad_motor_camera", "motor_0")
-    with BS.body_state_cpu_stack():
+    with articulated_cpu_stack():
         torch.manual_seed(0)
         env = _env("_test_quad_motor_camera", "env_with_obstacles", n=4)
         env.reset()
@@ -294,7 +277,7 @@ def test_rigid_robot_camera_on_a_fixed_link_equals_a_base_camera_with_the_link_f
 
 def test_unknown_parent_link_raises():
     _register_link_camera("_test_quad_no_such_link", "no_such_link")
-    with BS.body_state_cpu_stack():
+    with articulated_cpu_stack():
         with pytest.raises(ValueError, match=r"no_such_link.*base_link"):
             _env("_test_quad_no_such_link", "env_with_obstacles", n=2)
 
@@ -349,6 +332,6 @@ def levelling_check(env, dev):
 
 
 def test_gimbal_levels_the_camera():
-    with BS.body_state_cpu_stack():
+    with articulated_cpu_stack():
         torch.manual_seed(0)
         levelling_check(_env("base_quadrotor_with_gimbal_camera", "empty_env", n=4), "cpu")

@@ -1,5 +1,5 @@
 """Torque-driven (effort-mode) joints of articulated robots on the CPU (DESIGN.md "Articulated robots", "Torque-driven joints"): the
-step of art_env_step<M, NB, IMU, true> (host shadow, tests/csrc/articulated_effort_shadow.cu) against oracle/articulated_effort_oracle.py,
+step of art_env_step<M, NB, IMU, true> (host shadow, tests/csrc/articulated_shadow.cu) against oracle/articulated_effort_oracle.py,
 the oracle itself against articulated_oracle, momentum conservation, an analytic two-body case and its clamp, and the host layer
 (URDF, ArticulationSpec, Hp1Engine, EnvManager) on the CPU stack."""
 import ctypes as C
@@ -17,11 +17,10 @@ from oracle import articulated_imu_oracle as IO
 from oracle import articulated_oracle as AO
 
 from . import _hp1_common as H
-from ._cpu_stack_articulated import CpuArticulatedHp1Engine
-from ._cpu_stack_articulated_effort import CpuEffortHp1Engine, effort_cpu_stack
+from ._cpu_stack_articulated import CpuArticulatedHp1Engine, articulated_cpu_stack
 from .test_articulated_cpu import (_urdf, check_substep, load_inputs, morphy_compliant, oracle_state, random_art, random_root, shaped_art,
                                    substep_inputs, table_of)
-from .test_articulated_imu_cpu import _limit_crossing, gimbal_quad, sass_functions
+from .test_articulated_imu_cpu import _limit_crossing, gimbal_quad
 
 RES = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "aerial_gym_simulator_b200", "resources", "robots")
 
@@ -40,7 +39,7 @@ def effort_inputs(art, N, seed, over=1.5):
 
 def run_effort(spec, art, inp, effort, physics_steps=1, imu_body=None):
     n = inp["root"].shape[0]
-    eng = CpuEffortHp1Engine(spec, n, per_env_params="all", articulation=art, imu_body=imu_body)
+    eng = CpuArticulatedHp1Engine(spec, n, per_env_params="all", articulation=art, imu_body=imu_body)
     load_inputs(eng, inp)
     if eng.dof_actuation_force is not None:  # None without an effort DOF (a one-body tree)
         eng.dof_actuation_force.copy_(effort)
@@ -324,7 +323,7 @@ def _env(robot, env_name="empty_env", n=4, **args):
 
 
 def test_env_publishes_the_tensor_only_for_effort_robots():
-    with effort_cpu_stack():
+    with articulated_cpu_stack():
         torch.manual_seed(0)
         env = _env("base_quadrotor_with_torque_gimbal")
         gtd = env.global_tensor_dict
@@ -345,7 +344,7 @@ def test_env_publishes_the_tensor_only_for_effort_robots():
 
 def test_torque_moves_the_gimbal_and_the_base_reacts():
     """a constant roll torque on the hovering quad: the roll stage spins up one way, the base the other"""
-    with effort_cpu_stack():
+    with articulated_cpu_stack():
         torch.manual_seed(0)
         env = _env("base_quadrotor_with_torque_gimbal", n=2)
         env.spec.enable_disturbance = False
@@ -361,63 +360,3 @@ def test_torque_moves_the_gimbal_and_the_base_reacts():
         assert qd[0] > 0 and qd[1] < 0
         w = gtd["robot_angvel"]
         assert torch.sign(w[:, 0]).tolist() == [-1.0, 1.0]
-
-
-# ---- machine code ----------------------------------------------------------------------------------------------------------------
-# -Xptxas -v of the eight instantiations of articulated_step_effort_kernel<M, NB, IMU> (CUDA 12.9, sm_90a): registers per thread.  The
-# stack frame is the per-body arrays of the ABA, in local memory by design (articulated.cu): 3,312 B at NB = 9, 5,856 B at NB = 16, the
-# same as articulated_step_kernel's.  No spills.
-EFFORT_KERNEL_REGS = {(4, 9, 0): 158, (4, 16, 0): 158, (8, 9, 0): 167, (8, 16, 0): 167,
-                      (4, 9, 1): 158, (4, 16, 1): 158, (8, 9, 1): 167, (8, 16, 1): 167}
-EFFORT_KERNEL_STACK = {9: 3312, 16: 5856}
-# normalised SASS (test_articulated_imu_cpu.sass_functions), md5, of every step kernel articulated.cu had before the effort entry point
-PARENT_SASS = {
-    "articulated_step_kernelILi4ELi16E": "61f12510a9b31d109fae04dc1a814d87",
-    "articulated_step_kernelILi4ELi9E": "efbd4a3c22e2ad0447001440b6c8ac27",
-    "articulated_step_kernelILi8ELi16E": "4d833f5c266d542fe19e29d2b82ef233",
-    "articulated_step_kernelILi8ELi9E": "c2086c00bb11078baa2a0b9cc19015ce",
-    "articulated_step_imu_kernelILi4ELi16E": "126c2d9df2119902e827c3866d83e9fb",
-    "articulated_step_imu_kernelILi4ELi9E": "2b321c922eed32aa91bc91d3594f5433",
-    "articulated_step_imu_kernelILi8ELi16E": "f4eb229df3dcb4a243ca0d7daecea392",
-    "articulated_step_imu_kernelILi8ELi9E": "8418465ed540f9c3753c25a8ffefbfff",
-    "articulated_body_state_kernelILi16E": "49fabc56648bbeedb676825c9dfce8b7",
-    "articulated_body_state_kernelILi9E": "d6ab5ca7ca0215f6f63b3496123fa2d8",
-}
-
-
-@pytest.fixture(scope="module")
-def articulated_unit():
-    import subprocess
-    import tempfile
-
-    from aerial_gym_simulator_b200 import _build
-    src = os.path.join(_build.CSRC, "articulated.cu")
-    with tempfile.TemporaryDirectory() as d:
-        obj = os.path.join(d, "articulated.o")
-        r = subprocess.run([_build._nvcc()] + _build.NVCC_FLAGS + ["-Xptxas", "-v", "-c", src, "-o", obj], capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr
-        sass = subprocess.run([_build.cuda_tool("cuobjdump"), "-sass", obj], capture_output=True, text=True, check=True).stdout
-    return r.stderr, sass
-
-
-def test_effort_kernels_have_no_spills(articulated_unit):
-    import re
-    log, _ = articulated_unit
-    blocks = re.findall(r"Compiling entry function '(\S+)'.*?\n.*?(\d+) bytes stack frame, (.*?spill loads)\n.*?Used (\d+) registers", log,
-                        re.S)
-    found = {}
-    for f, stack, info, regs in blocks:
-        m = re.search(r"articulated_step_effort_kernelILi(\d)ELi(\d+)ELb(\d)E", f)
-        if m:
-            assert info == "0 bytes spill stores, 0 bytes spill loads", (f, info)
-            assert int(stack) == EFFORT_KERNEL_STACK[int(m.group(2))], (f, stack)
-            found[(int(m.group(1)), int(m.group(2)), int(m.group(3)))] = int(regs)
-    assert found == EFFORT_KERNEL_REGS, found
-
-
-def test_pre_existing_kernels_keep_their_sass(articulated_unit):
-    _, sass = articulated_unit
-    h = sass_functions(sass)
-    for key, md5 in PARENT_SASS.items():
-        hits = [v for k, v in h.items() if key in k and "effort" not in k]
-        assert hits == [md5], (key, hits)

@@ -1,18 +1,13 @@
 """The IMU on a link of an articulated robot, on the CPU (DESIGN.md "Articulated robots", "IMU on a link"): the IMU input of
-art_env_step<M, NB, true> (host shadow, tests/csrc/articulated_imu_shadow.cu) against oracle/articulated_imu_oracle.py, the oracle
+art_env_step<M, NB, true> (host shadow, tests/csrc/articulated_shadow.cu) against oracle/articulated_imu_oracle.py, the oracle
 itself against central differences, momentum balance and the rigid path, and the host layer (EnvManager, IMUSensor) on the CPU stack."""
 import ctypes as C
-import hashlib
-import os
-import re
-import subprocess
-import tempfile
 
 import numpy as np
 import pytest
 import torch
 
-from aerial_gym_simulator_b200 import _build, _lib
+from aerial_gym_simulator_b200 import _lib
 from oracle import articulated_body_state_oracle as BO
 from oracle import articulated_imu_oracle as IO
 from oracle import articulated_oracle as AO
@@ -20,8 +15,7 @@ from oracle import aux_oracle as XO
 from oracle import hp1_oracle as HO
 
 from . import _hp1_common as H
-from ._cpu_stack_articulated import CpuArticulatedHp1Engine
-from ._cpu_stack_articulated_imu import CpuImuHp1Engine, imu_cpu_stack
+from ._cpu_stack_articulated import CpuArticulatedHp1Engine, articulated_cpu_stack
 from .test_articulated_body_state_cpu import gimbal_levelling
 from .test_articulated_cpu import RTOL, load_inputs, morphy_compliant, oracle_state, random_art, random_root, shaped_art, \
     substep_inputs, table_of
@@ -82,7 +76,7 @@ def imu_tolerance(table, b, root, q, qd, a0, qdd, grav):
 
 def run_shadow(spec, art, b, inp, physics_steps=1):
     n = inp["root"].shape[0]
-    eng = CpuImuHp1Engine(spec, n, per_env_params="all", articulation=art, imu_body=b)
+    eng = CpuArticulatedHp1Engine(spec, n, per_env_params="all", articulation=art, imu_body=b)
     load_inputs(eng, inp)
     eng.physics_step(inp["actions"], disturbance=inp["dist"], physics_steps=physics_steps)
     return eng
@@ -184,7 +178,7 @@ def test_last_substep_start_and_zero_steps():
     two = CpuArticulatedHp1Engine(spec, 32, per_env_params="all", articulation=art)
     load_inputs(two, inp)
     two.physics_step(inp["actions"], disturbance=inp["dist"], physics_steps=2)
-    one = CpuImuHp1Engine(spec, 32, per_env_params="all", articulation=art, imu_body=2)
+    one = CpuArticulatedHp1Engine(spec, 32, per_env_params="all", articulation=art, imu_body=2)
     for k in ("root_state", "motor_thrust", "dof_state", "dof_position_setpoint", "dof_velocity_setpoint", "tau_inc", "tau_dec", "k_thrust",
               "K_pos", "K_vel", "K_rot", "K_angvel"):
         getattr(one, k).copy_(getattr(two, k))
@@ -332,7 +326,7 @@ def test_measurement_is_imu_update_of_the_oracle_force_input(world_frame):
     from aerial_gym_simulator_b200.config import robot_config as rc
     _register(f"_test_morphy_imu_motor_{int(world_frame)}", rc.MorphyCompliantCfg, "arm_motor_0", world_frame=world_frame)
     n = 16
-    with imu_cpu_stack():
+    with articulated_cpu_stack():
         torch.manual_seed(0)
         env = _env(f"_test_morphy_imu_motor_{int(world_frame)}", n=n)
         env.spec.enable_disturbance = False
@@ -388,7 +382,7 @@ def test_hovering_morphy_reads_gravity_along_body_z():
     scale with the arm's lever (the motor 0.07 m beyond the flap hinge, the hinge 0.1 m out) times the arm-to-base mass ratio, and
     the base's tilt, g (1 - cos)"""
     from aerial_gym_simulator_b200.utils.math import quat_mul
-    with imu_cpu_stack():
+    with articulated_cpu_stack():
         torch.manual_seed(0)
         env = _env("morphy_compliant_imu", n=16)
         env.spec.enable_disturbance = False
@@ -431,7 +425,7 @@ def test_gimbal_camera_imu_reads_the_specific_force_in_the_levelled_frame():
     _register("_test_gimbal_base_imu", rc.BaseQuadWithGimbalCameraCfg, "base_link", **exact)
     _register("_test_gimbal_cam_imu", rc.BaseQuadWithGimbalCameraImuCfg, "gimbal_camera_link", **exact)
     out = {}
-    with imu_cpu_stack():
+    with articulated_cpu_stack():
         for name in ("_test_gimbal_base_imu", "_test_gimbal_cam_imu"):
             torch.manual_seed(0)
             env = _env(name, n=4)
@@ -457,7 +451,7 @@ def test_parent_link_on_a_rigid_robot_only_folds_the_orientation():
     from aerial_gym_simulator_b200.config import robot_config as rc
     _register("_test_quad_imu_motor", rc.BaseQuadWithImuCfg, "motor_0")
     meas = {}
-    with imu_cpu_stack():
+    with articulated_cpu_stack():
         for name in ("base_quadrotor_with_imu", "_test_quad_imu_motor"):
             torch.manual_seed(0)
             env = _env(name, n=8)
@@ -478,7 +472,7 @@ def test_parent_link_on_a_rigid_robot_only_folds_the_orientation():
 
 def test_link_fold_after_every_draw():
     from aerial_gym_simulator_b200.utils.math import quat_mul
-    with imu_cpu_stack():
+    with articulated_cpu_stack():
         torch.manual_seed(0)
         env = _env("base_quadrotor_with_gimbal_camera_imu", n=8)
         imu = env.imu
@@ -493,7 +487,7 @@ def test_argument_validation():
     _register("_test_morphy_imu_nolink", rc.MorphyCompliantCfg, None)
     _register("_test_morphy_imu_badlink", rc.MorphyCompliantCfg, "no_such_link")
     _register("_test_morphy_imu_massless", rc.MorphyCompliantCfg, "connecting_link_0")
-    with imu_cpu_stack():
+    with articulated_cpu_stack():
         with pytest.raises(ValueError, match="joint reaction forces.*name the link with imu_config.parent_link"):
             _env("_test_morphy_imu_nolink")
         with pytest.raises(ValueError, match=r"no_such_link.*base_link"):
@@ -518,65 +512,3 @@ def test_argument_validation():
     with pytest.raises(ValueError, match="articulated"):
         from aerial_gym_simulator_b200.hp1 import Hp1Engine
         Hp1Engine._init_imu(type("E", (), {"articulation": None})(), 0)
-
-
-# ---- machine code ----------------------------------------------------------------------------------------------------------------
-# -Xptxas -v of the four instantiations of articulated_step_imu_kernel (CUDA 12.9, sm_90a): registers per thread.  The stack frame is
-# the per-body arrays of the ABA, in local memory by design (articulated.cu), the same size as articulated_step_kernel's.
-IMU_KERNEL_REGS = {(4, 9): 158, (4, 16): 158, (8, 9): 166, (8, 16): 166}
-# normalised SASS (tools/sass_hash.py's idea, per function: comment lines and addresses dropped, encodings kept, the anonymous
-# namespace's per-file hash masked) of every kernel articulated.cu had before the IMU entry point, md5
-PARENT_SASS = {
-    "articulated_body_state_kernelILi16E": "49fabc56648bbeedb676825c9dfce8b7",
-    "articulated_body_state_kernelILi9E": "d6ab5ca7ca0215f6f63b3496123fa2d8",
-    "articulated_step_kernelILi8ELi16E": "4d833f5c266d542fe19e29d2b82ef233",
-    "articulated_step_kernelILi8ELi9E": "c2086c00bb11078baa2a0b9cc19015ce",
-    "articulated_step_kernelILi4ELi16E": "61f12510a9b31d109fae04dc1a814d87",
-    "articulated_step_kernelILi4ELi9E": "efbd4a3c22e2ad0447001440b6c8ac27",
-}
-
-
-@pytest.fixture(scope="module")
-def articulated_unit():
-    src = os.path.join(_build.CSRC, "articulated.cu")
-    with tempfile.TemporaryDirectory() as d:
-        obj = os.path.join(d, "articulated.o")
-        r = subprocess.run([_build._nvcc()] + _build.NVCC_FLAGS + ["-Xptxas", "-v", "-c", src, "-o", obj], capture_output=True, text=True)
-        assert r.returncode == 0, r.stderr
-        sass = subprocess.run([_build.cuda_tool("cuobjdump"), "-sass", obj], capture_output=True, text=True, check=True).stdout
-    return r.stderr, sass
-
-
-def sass_functions(txt):
-    out, cur = {}, None
-    for line in txt.splitlines():
-        m = re.match(r"\s+Function : (\S+)", line)
-        if m:
-            cur = re.sub(r"_GLOBAL__N__\w+?_cu_\w{8}", "ANON", m.group(1))
-            out[cur] = []
-            continue
-        s = line.strip()
-        if cur is None or not s or s.startswith(("//", "...", ".")):
-            continue
-        out[cur].append(re.sub(r"/\*[0-9a-f]{4,}\*/", "", s))
-    return {k: hashlib.md5("\n".join(v).encode()).hexdigest() for k, v in out.items()}
-
-
-def test_imu_kernels_have_no_spills(articulated_unit):
-    log, _ = articulated_unit
-    blocks = re.findall(r"Compiling entry function '(\S+)'.*?\n(.*?spill loads)\n.*?Used (\d+) registers", log, re.S)
-    found = {}
-    for f, info, regs in blocks:
-        m = re.search(r"articulated_step_imu_kernelILi(\d)ELi(\d+)E", f)
-        if m:
-            assert "0 bytes spill stores, 0 bytes spill loads" in info, (f, info)
-            found[(int(m.group(1)), int(m.group(2)))] = int(regs)
-    assert found == IMU_KERNEL_REGS, found
-
-
-def test_pre_existing_kernels_keep_their_sass(articulated_unit):
-    _, sass = articulated_unit
-    h = sass_functions(sass)
-    for key, md5 in PARENT_SASS.items():
-        hits = [v for k, v in h.items() if key in k and "imu" not in k]
-        assert hits == [md5], (key, hits)

@@ -1,11 +1,10 @@
 """Joint force sensing of articulated robots on the CPU (DESIGN.md "Articulated robots", "Joint force sensing"): joint_wrench and
-dof_force of art_env_step<M, NB, true, true, true> (host shadow, tests/csrc/articulated_joint_force_shadow.cu) against
+dof_force of art_env_step<M, NB, true, true, true> (host shadow, tests/csrc/articulated_shadow.cu) against
 oracle/articulated_joint_force_oracle.py, the oracle's own checks (the dof_force identity, the base's Newton-Euler balance, a hanging
 pendulum, a one-body tree), bit identity of the state with the plain, IMU and effort steps, static loads at hover, and the host layer
 (Hp1Engine, EnvManager, the C ABI) on the CPU stack."""
 import ctypes as C
 import dataclasses
-import re
 
 import numpy as np
 import pytest
@@ -18,14 +17,11 @@ from oracle import articulated_joint_force_oracle as JO
 from oracle import hp1_oracle as HO
 
 from . import _hp1_common as H
-from ._cpu_stack_articulated import CpuArticulatedHp1Engine
-from ._cpu_stack_articulated_effort import CpuEffortHp1Engine
-from ._cpu_stack_articulated_imu import CpuImuHp1Engine
-from ._cpu_stack_articulated_joint_force import CpuJointForceHp1Engine, joint_force_cpu_stack
+from ._cpu_stack_articulated import CpuArticulatedHp1Engine, articulated_cpu_stack
 from .test_articulated_cpu import RTOL, load_inputs, morphy_compliant, oracle_state, random_art, random_root, shaped_art, substep_inputs, \
     table_of
-from .test_articulated_effort_cpu import articulated_unit, effort_inputs, with_modes  # noqa: F401 (articulated_unit is a fixture)
-from .test_articulated_imu_cpu import _depth, _limit_crossing, gimbal_quad, sass_functions
+from .test_articulated_effort_cpu import effort_inputs, with_modes
+from .test_articulated_imu_cpu import _depth, _limit_crossing, gimbal_quad
 
 EPS = float(np.finfo(np.float32).eps)
 ULPS = 8
@@ -34,7 +30,7 @@ STATE = ("root_state", "motor_thrust", "dof_state") + CpuArticulatedHp1Engine.DE
 
 def run_jf(spec, art, inp, physics_steps=1, imu_body=None, effort=None):
     n = inp["root"].shape[0]
-    eng = CpuJointForceHp1Engine(spec, n, per_env_params="all", articulation=art, imu_body=imu_body, joint_force=True)
+    eng = CpuArticulatedHp1Engine(spec, n, per_env_params="all", articulation=art, imu_body=imu_body, joint_force=True)
     load_inputs(eng, inp)
     if eng.dof_actuation_force is not None:
         eng.dof_actuation_force.copy_(effort)
@@ -282,7 +278,7 @@ def test_state_and_imu_are_bit_identical_to_the_other_steps():
         load_inputs(plain, inp)
         plain.physics_step(inp["actions"], disturbance=inp["dist"], physics_steps=steps)
         jf = run_jf(spec, morphy, inp, physics_steps=steps)
-        imu = CpuImuHp1Engine(spec, 32, per_env_params="all", articulation=morphy, imu_body=4)
+        imu = CpuArticulatedHp1Engine(spec, 32, per_env_params="all", articulation=morphy, imu_body=4)
         load_inputs(imu, inp)
         imu.physics_step(inp["actions"], disturbance=inp["dist"], physics_steps=steps)
         jfi = run_jf(spec, morphy, inp, physics_steps=steps, imu_body=4)
@@ -293,7 +289,7 @@ def test_state_and_imu_are_bit_identical_to_the_other_steps():
         assert torch.equal(jf.joint_wrench, jfi.joint_wrench) and torch.equal(jf.dof_force, jfi.dof_force)
         inp = _limit_crossing(substep_inputs(spec, tg, 32, 30 + steps), tg)
         e = effort_inputs(tg, 32, 31)
-        eff = CpuEffortHp1Engine(spec, 32, per_env_params="all", articulation=tg, imu_body=2)
+        eff = CpuArticulatedHp1Engine(spec, 32, per_env_params="all", articulation=tg, imu_body=2)
         load_inputs(eff, inp)
         eff.dof_actuation_force.copy_(e)
         eff.physics_step(inp["actions"], disturbance=inp["dist"], physics_steps=steps)
@@ -314,7 +310,7 @@ def test_last_substep_start():
     two = CpuArticulatedHp1Engine(spec, 32, per_env_params="all", articulation=art)
     load_inputs(two, inp)
     two.physics_step(inp["actions"], disturbance=inp["dist"], physics_steps=2)
-    one = CpuJointForceHp1Engine(spec, 32, per_env_params="all", articulation=art, joint_force=True)
+    one = CpuArticulatedHp1Engine(spec, 32, per_env_params="all", articulation=art, joint_force=True)
     for k in ("root_state", "motor_thrust", "dof_state", "dof_position_setpoint", "dof_velocity_setpoint", "tau_inc", "tau_dec", "k_thrust",
               "K_pos", "K_vel", "K_rot", "K_angvel"):
         getattr(one, k).copy_(getattr(two, k))
@@ -373,7 +369,7 @@ def test_hovering_morphy_flap_joints_carry_the_static_load():
     axis, both in the flap body's frame"""
     from aerial_gym_simulator_b200.config import robot_config as rc
     name = _register("_test_morphy_jf", rc.MorphyCompliantCfg)
-    with joint_force_cpu_stack():
+    with articulated_cpu_stack():
         torch.manual_seed(0)
         env, gtd = _hover(name)
         b = env.robot.bodies
@@ -399,7 +395,7 @@ def test_hovering_gimbal_stages_carry_their_weight_and_no_axis_torque():
     stage's weight times its 6 cm drop"""
     from aerial_gym_simulator_b200.config import robot_config as rc
     name = _register("_test_gimbal_jf", rc.BaseQuadWithGimbalCameraCfg)
-    with joint_force_cpu_stack():
+    with articulated_cpu_stack():
         torch.manual_seed(0)
         env, gtd = _hover(name)
         b = env.robot.bodies
@@ -417,7 +413,7 @@ def test_hovering_gimbal_stages_carry_their_weight_and_no_axis_torque():
 def test_env_publishes_the_tensors_only_with_the_flag():
     from aerial_gym_simulator_b200.config import robot_config as rc
     names = [_register("_test_gimbal_jf2", rc.BaseQuadWithGimbalCameraCfg), _register("_test_torque_gimbal_jf", rc.BaseQuadWithTorqueGimbalCfg)]
-    with joint_force_cpu_stack():
+    with articulated_cpu_stack():
         for robot in names:
             torch.manual_seed(0)
             env = _env(robot)
@@ -440,7 +436,7 @@ def test_env_publishes_the_tensors_only_with_the_flag():
 def test_rigid_robot_raises():
     from aerial_gym_simulator_b200.config import robot_config as rc
     name = _register("_test_quad_jf", rc.BaseQuadCfg)
-    with joint_force_cpu_stack():
+    with articulated_cpu_stack():
         with pytest.raises(ValueError, match="joint_force belongs to an articulated robot"):
             _env(name)
 
@@ -472,53 +468,3 @@ def test_c_abi_validation():
         assert call(1, C.byref(e), w=w, d=d) != 0 and b"joint_wrench/dof_force is NULL" in lib.agx_last_error()
     for w, d in ((jw.data_ptr() + 8, df.data_ptr()), (jw.data_ptr(), df.data_ptr() + 4)):
         assert call(1, C.byref(e), w=w, d=d) != 0 and b"16-byte aligned" in lib.agx_last_error()
-
-
-# ---- machine code ----------------------------------------------------------------------------------------------------------------
-# -Xptxas -v of the four instantiations of articulated_step_joint_force_kernel<M, NB> (CUDA 12.9, sm_90a): registers per thread.  The
-# stack frame is the per-body arrays of the ABA, in local memory by design (articulated.cu), the same as articulated_step_kernel's.
-JF_KERNEL_REGS = {(4, 9): 165, (4, 16): 165, (8, 9): 168, (8, 16): 168}
-JF_KERNEL_STACK = {9: 3312, 16: 5856}
-# normalised SASS (test_articulated_imu_cpu.sass_functions), md5, of every kernel articulated.cu had before the joint-force entry point
-PARENT_SASS = {
-    "articulated_step_kernelILi4ELi16E": "61f12510a9b31d109fae04dc1a814d87",
-    "articulated_step_kernelILi4ELi9E": "efbd4a3c22e2ad0447001440b6c8ac27",
-    "articulated_step_kernelILi8ELi16E": "4d833f5c266d542fe19e29d2b82ef233",
-    "articulated_step_kernelILi8ELi9E": "c2086c00bb11078baa2a0b9cc19015ce",
-    "articulated_step_imu_kernelILi4ELi16E": "126c2d9df2119902e827c3866d83e9fb",
-    "articulated_step_imu_kernelILi4ELi9E": "2b321c922eed32aa91bc91d3594f5433",
-    "articulated_step_imu_kernelILi8ELi16E": "f4eb229df3dcb4a243ca0d7daecea392",
-    "articulated_step_imu_kernelILi8ELi9E": "8418465ed540f9c3753c25a8ffefbfff",
-    "articulated_step_effort_kernelILi4ELi16ELb0E": "09c0d3e7332544ce33a23224720c7ea1",
-    "articulated_step_effort_kernelILi4ELi16ELb1E": "9579cc186f99b4fd0882a770a5f271e5",
-    "articulated_step_effort_kernelILi4ELi9ELb0E": "abd31654971564ffba13ba49beb4fec6",
-    "articulated_step_effort_kernelILi4ELi9ELb1E": "f6b6f80c1bcce608057bcdea4b8ec6cb",
-    "articulated_step_effort_kernelILi8ELi16ELb0E": "3460f725d21829e0b968c1d33a994119",
-    "articulated_step_effort_kernelILi8ELi16ELb1E": "1574c81ff97a7ac7fc0231afe3a3f2a2",
-    "articulated_step_effort_kernelILi8ELi9ELb0E": "c3c8b9d43a5e98e00d872969082d91ee",
-    "articulated_step_effort_kernelILi8ELi9ELb1E": "a32e11ab74110bf4d33d9e436db96c31",
-    "articulated_body_state_kernelILi16E": "49fabc56648bbeedb676825c9dfce8b7",
-    "articulated_body_state_kernelILi9E": "d6ab5ca7ca0215f6f63b3496123fa2d8",
-}
-
-
-def test_joint_force_kernels_have_no_spills(articulated_unit):  # noqa: F811
-    log, _ = articulated_unit
-    blocks = re.findall(r"Compiling entry function '(\S+)'.*?\n.*?(\d+) bytes stack frame, (.*?spill loads)\n.*?Used (\d+) registers", log,
-                        re.S)
-    found = {}
-    for f, stack, info, regs in blocks:
-        m = re.search(r"articulated_step_joint_force_kernelILi(\d)ELi(\d+)E", f)
-        if m:
-            assert info == "0 bytes spill stores, 0 bytes spill loads", (f, info)
-            assert int(stack) == JF_KERNEL_STACK[int(m.group(2))], (f, stack)
-            found[(int(m.group(1)), int(m.group(2)))] = int(regs)
-    assert found == JF_KERNEL_REGS, found
-
-
-def test_pre_existing_kernels_keep_their_sass(articulated_unit):  # noqa: F811
-    _, sass = articulated_unit
-    h = sass_functions(sass)
-    for key, md5 in PARENT_SASS.items():
-        hits = [v for k, v in h.items() if key in k]
-        assert hits == [md5], (key, hits)

@@ -1,7 +1,7 @@
 """Per-body state of articulated robots on the H100: agx_hp1_articulated_body_state against the float64 body_states() of
 oracle/articulated_body_state_oracle.py and its host shadow, CUDA-graph step mode against launch mode for robot_body_state_tensor, and the gimbal
 quadrotor's camera and levelling in an obstacle env.  With --gpu-dryrun the same text runs on the host shadow
-(tests/_cpu_stack_body_state.py)."""
+(tests/_cpu_stack_articulated.py)."""
 import contextlib
 import ctypes as C
 
@@ -10,7 +10,8 @@ import pytest
 import torch
 
 from aerial_gym_simulator_b200 import _lib
-from tests import _cpu_stack_body_state as BS
+from tests import _articulated_shadow
+from tests._cpu_stack_articulated import articulated_twin_for_dryrun
 from tests.test_articulated_body_state_cpu import _cases, _check_rows, gimbal_camera_check, levelling_check
 from tests.test_articulated_cpu import morphy_compliant, random_art, table_of
 
@@ -22,7 +23,7 @@ DEV = "cuda:0"
 def _body_state_twin():
     """with --gpu-dryrun (tests/conftest.py has set DEV to "cpu" and entered the CPU stack) EnvManager's engine is the CPU twin that
     publishes the body states; on the GPU nothing changes"""
-    with BS.body_state_twin_for_dryrun() if DEV == "cpu" else contextlib.nullcontext():
+    with articulated_twin_for_dryrun() if DEV == "cpu" else contextlib.nullcontext():
         yield
 
 
@@ -36,7 +37,7 @@ def _launch(art, roots, dof, stride):
     s.dof_state = dof_t.data_ptr()
     out = torch.full((N, s.num_bodies, 13), float("nan"), device=DEV)
     if DEV == "cpu":
-        BS.body_state(s, root_t, out)
+        _articulated_shadow.body_state(s, root_t, out)
     else:
         lib = _lib.load()
         _lib.check(lib.agx_hp1_articulated_body_state(C.byref(s), N, root_t.data_ptr(), stride, out.data_ptr(),
@@ -63,7 +64,7 @@ def test_kernel_matches_oracle_and_shadow(B):
         dof_t = torch.tensor(dofs).contiguous()
         ss.dof_state = dof_t.data_ptr()
         sh_t = torch.from_numpy(sh)
-        BS.body_state(ss, torch.tensor(roots), sh_t)
+        _articulated_shadow.body_state(ss, torch.tensor(roots), sh_t)
         assert np.isfinite(got).all()
         # device vs shadow: positions / velocities by value, rotations as matrices
         d = np.abs(got - sh)

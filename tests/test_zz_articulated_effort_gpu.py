@@ -1,7 +1,7 @@
 """Torque-driven joints of articulated robots on the H100: agx_hp1_articulated_step_effort in its eight instantiations against the host
 shadow and the float64 oracle (oracle/articulated_effort_oracle.py), momentum balance on the device, CUDA-graph step mode against
 launch mode, the clamp, and base_quadrotor_with_torque_gimbal levelling its camera with a torque law in an obstacle env.  With
---gpu-dryrun the same text runs on the host shadow (tests/_cpu_stack_articulated_effort.py)."""
+--gpu-dryrun the same text runs on the host shadow (tests/_cpu_stack_articulated.py)."""
 import contextlib
 import ctypes as C
 
@@ -10,8 +10,8 @@ import pytest
 import torch
 
 from aerial_gym_simulator_b200.hp1 import Hp1Engine
-from tests import _cpu_stack_articulated_effort as CE
 from tests import _hp1_common as H
+from tests._cpu_stack_articulated import CpuArticulatedHp1Engine, articulated_twin_for_dryrun
 from tests.test_articulated_cpu import check_substep, load_inputs, morphy_compliant, shaped_art, substep_inputs
 from tests.test_articulated_effort_cpu import effort_inputs, reference_effort_substep, with_modes
 from tests.test_articulated_imu_cpu import _limit_crossing, check_imu, gimbal_quad
@@ -22,14 +22,14 @@ DEV = "cuda:0"
 
 @pytest.fixture(autouse=True)
 def _effort_twin():
-    with CE.effort_twin_for_dryrun() if DEV == "cpu" else contextlib.nullcontext():
+    with articulated_twin_for_dryrun() if DEV == "cpu" else contextlib.nullcontext():
         yield
 
 
 def _engine(spec, n, art, imu_body=None, dev=None):
     dev = DEV if dev is None else dev
     if dev == "cpu":
-        eng = CE.CpuEffortHp1Engine(spec, n, per_env_params="all", articulation=art, imu_body=imu_body)
+        eng = CpuArticulatedHp1Engine(spec, n, per_env_params="all", articulation=art, imu_body=imu_body)
     else:
         eng = Hp1Engine(spec, n, dev, per_env_params="all", articulation=art, imu_body=imu_body)
     if eng._effort is None:  # a one-body tree has no DOF to put in effort mode: run the effort entry point with an empty table

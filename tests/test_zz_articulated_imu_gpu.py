@@ -1,7 +1,7 @@
 """The IMU on a link of an articulated robot on the H100: agx_hp1_articulated_step_imu in its four instantiations against the host
 shadow and the float64 oracle (oracle/articulated_imu_oracle.py), its state outputs against agx_hp1_articulated_step's,
 momentum balance over one launch per body, CUDA-graph step mode against launch mode with imu_measurement, and the gimbal IMU end to
-end.  With --gpu-dryrun the same text runs on the host shadow (tests/_cpu_stack_articulated_imu.py)."""
+end.  With --gpu-dryrun the same text runs on the host shadow (tests/_cpu_stack_articulated.py)."""
 import contextlib
 
 import numpy as np
@@ -9,9 +9,8 @@ import pytest
 import torch
 
 from aerial_gym_simulator_b200.hp1 import Hp1Engine
-from tests import _cpu_stack_articulated_imu as CI
 from tests import _hp1_common as H
-from tests._cpu_stack_articulated import CpuArticulatedHp1Engine
+from tests._cpu_stack_articulated import CpuArticulatedHp1Engine, articulated_twin_for_dryrun
 from tests.test_articulated_cpu import check_substep, load_inputs, morphy_compliant, reference_substep, shaped_art, substep_inputs
 from tests.test_articulated_imu_cpu import check_imu
 
@@ -21,13 +20,13 @@ DEV = "cuda:0"
 
 @pytest.fixture(autouse=True)
 def _imu_twin():
-    with CI.imu_twin_for_dryrun() if DEV == "cpu" else contextlib.nullcontext():
+    with articulated_twin_for_dryrun() if DEV == "cpu" else contextlib.nullcontext():
         yield
 
 
 def _engine(spec, n, art, b):
     if DEV == "cpu":
-        return CI.CpuImuHp1Engine(spec, n, per_env_params="all", articulation=art, imu_body=b)
+        return CpuArticulatedHp1Engine(spec, n, per_env_params="all", articulation=art, imu_body=b)
     return Hp1Engine(spec, n, DEV, per_env_params="all", articulation=art, imu_body=b)
 
 
@@ -70,7 +69,7 @@ def test_kernel_matches_shadow_and_oracle(M, B):
         ref, ok = reference_substep(eng, spec, art, inp, idx)
         check_substep(eng, spec, inp, ref, ok, idx)
         got = eng.imu_input.cpu()
-        sh = CI.CpuImuHp1Engine(spec, N, per_env_params="all", articulation=art, imu_body=b)
+        sh = CpuArticulatedHp1Engine(spec, N, per_env_params="all", articulation=art, imu_body=b)
         _step_cpu = (lambda e: (load_inputs(e, inp), e.physics_step(inp["actions"], disturbance=inp["dist"], physics_steps=1)))
         _step_cpu(sh)
         scale = sh.imu_input.abs().amax(0, keepdim=True) + 1e-6

@@ -1,7 +1,7 @@
 """Joint force sensing of articulated robots on the H100: agx_hp1_articulated_step_joint_force in its four instantiations against the
 host shadow and the float64 oracle (oracle/articulated_joint_force_oracle.py), the base's momentum balance on the device, the state
 against the plain kernel, CUDA-graph step mode against launch mode, and the clamp.  With --gpu-dryrun the same text runs on the host
-shadow (tests/_cpu_stack_articulated_joint_force.py)."""
+shadow (tests/_cpu_stack_articulated.py)."""
 import contextlib
 
 import numpy as np
@@ -9,7 +9,7 @@ import pytest
 import torch
 
 from aerial_gym_simulator_b200.hp1 import Hp1Engine
-from tests import _cpu_stack_articulated_joint_force as CJ
+from tests._cpu_stack_articulated import CpuArticulatedHp1Engine, articulated_twin_for_dryrun
 from tests import _hp1_common as H
 from tests.test_articulated_cpu import load_inputs, morphy_compliant, shaped_art, substep_inputs
 from tests.test_articulated_cpu import check_substep
@@ -24,14 +24,14 @@ STATE = ("root_state", "motor_thrust", "dof_state") + Hp1Engine.DERIVED
 
 @pytest.fixture(autouse=True)
 def _jf_twin():
-    with CJ.joint_force_twin_for_dryrun() if DEV == "cpu" else contextlib.nullcontext():
+    with articulated_twin_for_dryrun() if DEV == "cpu" else contextlib.nullcontext():
         yield
 
 
 def _engine(spec, n, art, imu_body=None, dev=None, joint_force=True):
     dev = DEV if dev is None else dev
     if dev == "cpu":
-        return CJ.CpuJointForceHp1Engine(spec, n, per_env_params="all", articulation=art, imu_body=imu_body, joint_force=joint_force)
+        return CpuArticulatedHp1Engine(spec, n, per_env_params="all", articulation=art, imu_body=imu_body, joint_force=joint_force)
     return Hp1Engine(spec, n, dev, per_env_params="all", articulation=art, imu_body=imu_body, joint_force=joint_force)
 
 
