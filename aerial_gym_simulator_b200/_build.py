@@ -18,6 +18,7 @@ UNITS = [
     ("hp1.cu", ["-prec-div=false", "-prec-sqrt=false"]),  # AGX_FAST_TRIG: 3x parity error -> off
     ("hp1_aux.cu", []),
     ("articulated.cu", []),
+    ("articulated_prismatic.cu", []),
     ("lidar_nav.cu", []),
     # device-RNG units: no FMA contraction, so "lo + (hi - lo) u" and the noise model round like their numpy oracles
     ("sensor_noise.cu", ["-fmad=false"]),

@@ -226,6 +226,11 @@ def load():
         "agx_hp1_articulated_step_joint_force": [C.POINTER(AgxHp1Config), C.POINTER(AgxHp1Buffers), C.POINTER(AgxArticulation),
                                                  C.POINTER(AgxJointEffort), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p],
         "agx_hp1_articulated_body_state": [C.POINTER(AgxArticulation), C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p],
+        "agx_hp1_articulated_step_prismatic": [C.POINTER(AgxHp1Config), C.POINTER(AgxHp1Buffers), C.POINTER(AgxArticulation),
+                                               C.c_uint32, C.POINTER(AgxJointEffort), C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                               C.c_void_p],
+        "agx_hp1_articulated_body_state_prismatic": [C.POINTER(AgxArticulation), C.c_uint32, C.c_int, C.c_void_p, C.c_int, C.c_void_p,
+                                                     C.c_void_p],
         "agx_hp1_reset": [C.POINTER(AgxHp1Config), C.POINTER(AgxHp1Buffers), C.c_void_p,
                           C.POINTER(AgxHp1ResetDraws), C.c_void_p],
         "agx_hp1_refresh": [C.POINTER(AgxHp1Config), C.POINTER(AgxHp1Buffers), C.c_int, C.c_void_p],

@@ -529,3 +529,25 @@ class BaseQuadWithTorqueGimbalCfg(BaseQuadWithGimbalCameraCfg):
 
     class joint_config(BaseQuadWithGimbalCameraCfg.joint_config):
         drive_mode = "effort"
+
+
+class BaseQuadWithSlidingPayloadCfg(BaseQuadCfg):
+    """base_quadrotor with a sliding payload (ours): quad_slider.urdf hangs payload_rail_joint, prismatic along the base x axis
+    within +-0.05 m, 3 cm below the base origin, and payload_link (0.05 kg, COM on the rail) on it -- a moving-mass robot.  The drive
+    acts on the relative motion of payload and airframe, whose reduced mass is mu = 0.05 x 0.25 / 0.30 = 0.042 kg: k = 10 N / m gives
+    w = sqrt(k / mu) = 15.5 rad/s (w dt = 0.155 at dt = 0.01) and d = 0.9 N s / m a damping ratio d / (2 sqrt(k mu)) = 0.70
+    (DESIGN.md "Articulated robots", "Prismatic joints").  Holding the payload at q* = 0.05 m takes m_p g q* = 0.025 N m of pitch
+    torque: a thrust difference of 0.19 N across the motors' 0.13 m lever arm, 13 % of a motor pair's hover thrust."""
+    class robot_asset(BaseQuadCfg.robot_asset):
+        file = "quad_slider.urdf"
+        name = "base_quadrotor_with_sliding_payload"
+
+    class joint_config:
+        # per DOF (payload_rail_joint: q in m, k in N / m, d in N s / m, drive_mode "effort" takes N); for a robot with several DOFs
+        # a scalar applies to all and a list gives one value per DOF, each in its own joint's units
+        stiffness = 10.0
+        damping = 0.9
+        min_init_dof_position = 0.0
+        max_init_dof_position = 0.0
+        min_init_dof_velocity = 0.0
+        max_init_dof_velocity = 0.0

@@ -181,9 +181,9 @@ AGX_DEV void art_joint_force(const AgxArticulation& art, int i, const M33& R, V3
 }
 
 // w_b = R_b^T w_b of body b without the dynamics (the IMU input of a launch with physics_steps = 0): the forward kinematics of
-// art_dynamics along the bodies 0..b
-template <int NB>
-AGX_DEV V3 art_body_angvel(const AgxArticulation& art, const EnvState& s, const float* q, const float* qd, int b) {
+// art_dynamics along the bodies 0..b.  PRISM: the joints of the bodies set in pmask are prismatic (art_dynamics' PRISM).
+template <int NB, bool PRISM = false>
+AGX_DEV V3 art_body_angvel(const AgxArticulation& art, const EnvState& s, const float* q, const float* qd, int b, uint32_t pmask = 0) {
     M33 R[NB];
     V3 W[NB];
     R[0] = quat_to_matrix(s.q);
@@ -192,6 +192,13 @@ AGX_DEV V3 art_body_angvel(const AgxArticulation& art, const EnvState& s, const 
         const int l = art.parent[i];
         const V3 ax = ld3(art.axis[i]);
         const M33 RJ = mul33(R[l], ld33(art.joint_R[i]));
+        if constexpr (PRISM) {
+            if ((pmask >> i) & 1u) {  // a slider turns nothing
+                R[i] = RJ;
+                W[i] = W[l];
+                continue;
+            }
+        }
         R[i] = mul33(RJ, axis_angle(ax, q[i - 1]));
         W[i] = W[l] + mul33v(RJ, ax) * qd[i - 1];
     }
@@ -209,11 +216,14 @@ AGX_DEV V3 art_body_angvel(const AgxArticulation& art, const EnvState& s, const 
 // EFFORT: the joints with eff->effort_dof[i] set are torque-driven: qs holds their tau_e and their k is 0, so the explicit force is
 // tau_e - d qd (d = the URDF damping alone, passive) and the pivot S^T I^A S + dt d.
 // JFORCE: where jw != NULL, also art_joint_force of every body i >= 1 into jw + 6 i and jdof + i - 1, and zeros into jw[0..5].
-template <int NB, bool IMU = false, bool EFFORT = false, bool JFORCE = false>
+// PRISM: the joint of every body i set in pmask is prismatic, a translation by q along its axis a = R_l joint_R_i axis_i: R_i =
+// R_l joint_R_i, P_i = P_l + R_l joint_p_i + a q and S_i = (0, a); its drive force is the same law in N, and its jdof entry is
+// axis_i . (the force of its jw row).  The other joints are stepped as without it.
+template <int NB, bool IMU = false, bool EFFORT = false, bool JFORCE = false, bool PRISM = false>
 AGX_DEV void art_dynamics(const AgxArticulation& art, const EnvState& s, const float* q, const float* qd, const float* qs,
                           const float* qds, float dt, V3 grav, int M, const float* thrust, V3 F_w, V3 T_w, float* a0, float* qdd,
                           int imu_body = 0, float* imu = nullptr, const AgxJointEffort* eff = nullptr, float* jw = nullptr,
-                          float* jdof = nullptr) {
+                          float* jdof = nullptr, uint32_t pmask = 0) {
     const int B = art.num_bodies;
     M33 R[NB];
     V3 P[NB];
@@ -227,10 +237,19 @@ AGX_DEV void art_dynamics(const AgxArticulation& art, const EnvState& s, const f
             const int l = art.parent[i];
             const V3 ax = ld3(art.axis[i]);
             const M33 RJ = mul33(R[l], ld33(art.joint_R[i]));
-            R[i] = mul33(RJ, axis_angle(ax, q[i - 1]));
-            P[i] = P[l] + mul33v(R[l], ld3(art.joint_p[i]));
-            const V3 aw = mul33v(RJ, ax);  // = R[i] ax
-            sv_set(S[i], aw, cross(P[i], aw));
+            bool slide = false;
+            if constexpr (PRISM) slide = (pmask >> i) & 1u;
+            if (slide) {
+                const V3 aw = mul33v(RJ, ax);
+                R[i] = RJ;
+                P[i] = P[l] + mul33v(R[l], ld3(art.joint_p[i])) + aw * q[i - 1];
+                sv_set(S[i], V3{0.0f, 0.0f, 0.0f}, aw);
+            } else {
+                R[i] = mul33(RJ, axis_angle(ax, q[i - 1]));
+                P[i] = P[l] + mul33v(R[l], ld3(art.joint_p[i]));
+                const V3 aw = mul33v(RJ, ax);  // = R[i] ax
+                sv_set(S[i], aw, cross(P[i], aw));
+            }
             float vj[6];
 #pragma unroll
             for (int k = 0; k < 6; ++k) vj[k] = S[i][k] * qd[i - 1];
@@ -315,6 +334,9 @@ AGX_DEV void art_dynamics(const AgxArticulation& art, const EnvState& s, const f
         for (int r = 0; r < 6; ++r) A[i][r] = ai[r] + S[i][r] * x;
         if constexpr (JFORCE) {
             if (jw) art_joint_force(art, i, R[i], P[i], IA[i], PA[i], A[i], jw + 6 * i, jdof + (i - 1));
+            if constexpr (PRISM) {
+                if (jw && ((pmask >> i) & 1u)) jdof[i - 1] = dot(ld3(art.axis[i]), ld3(jw + 6 * i));  // the force along the slide
+            }
         }
     }
     if constexpr (JFORCE) {
@@ -397,10 +419,12 @@ AGX_DEV void art_load_params(const AgxHp1Config& cfg, const AgxHp1Buffers& buf, 
 // JFORCE (with IMU and EFFORT): also the joint forces of the last sub-step into THIS env's rows, joint_wrench [B,6] and
 // dof_force [D] (art_dynamics' JFORCE; the kernel points them at shared memory), both zero with physics_steps = 0.  The IMU input is written only where imu_input != NULL, and an eff
 // without effort DOFs steps every DOF as the plain step does.  The state arithmetic is unchanged.
-template <int M, int NB, bool IMU = false, bool EFFORT = false, bool JFORCE = false>
+// PRISM (with JFORCE): the joints of the bodies set in pmask are prismatic (art_dynamics' PRISM), and the joint forces are written
+// only where joint_wrench != NULL.
+template <int M, int NB, bool IMU = false, bool EFFORT = false, bool JFORCE = false, bool PRISM = false>
 AGX_DEV void art_env_step(const AgxHp1Config& cfg, const AgxHp1Buffers& buf, const AgxArticulation& art, int env, int imu_body = 0,
                           float* imu_input = nullptr, const AgxJointEffort* eff = nullptr, float* joint_wrench = nullptr,
-                          float* dof_force = nullptr) {
+                          float* dof_force = nullptr, uint32_t pmask = 0) {
     EnvParams<M> p;
     art_load_params<M>(cfg, buf, env, p);
     const int A = cfg.num_actions;
@@ -464,21 +488,21 @@ AGX_DEV void art_env_step(const AgxHp1Config& cfg, const AgxHp1Buffers& buf, con
         float a0[6];
         const bool last = step + 1 == cfg.physics_steps;
         float* imu = (IMU && last && (!JFORCE || imu_input)) ? imu_input + (size_t)env * 9 : nullptr;
-        art_dynamics<NB, IMU, EFFORT, JFORCE>(art, s, q, qd, qs, qds, cfg.dt, grav, M, p.thrust, quat_rotate(s.q, df),
-                                              quat_rotate(s.q, dtq), a0, qdd, imu_body, imu, eff, (JFORCE && last) ? joint_wrench : nullptr,
-                                              dof_force);
+        art_dynamics<NB, IMU, EFFORT, JFORCE, PRISM>(art, s, q, qd, qs, qds, cfg.dt, grav, M, p.thrust, quat_rotate(s.q, df),
+                                                     quat_rotate(s.q, dtq), a0, qdd, imu_body, imu, eff,
+                                                     (JFORCE && last) ? joint_wrench : nullptr, dof_force, pmask);
         art_integrate(cfg, art, s, a0, q, qd, qdd);
     }
     if (cfg.physics_steps == 0) d = update_states(s);
     if constexpr (JFORCE) {
-        if (cfg.physics_steps == 0) {
+        if (cfg.physics_steps == 0 && (!PRISM || joint_wrench)) {
             for (int k = 0; k < 6 * art.num_bodies; ++k) joint_wrench[k] = 0.0f;
             for (int j = 0; j < D; ++j) dof_force[j] = 0.0f;
         }
     }
     if constexpr (IMU) {
         if (cfg.physics_steps == 0 && (!JFORCE || imu_input)) {
-            const V3 wb = art_body_angvel<NB>(art, s, q, qd, imu_body);
+            const V3 wb = art_body_angvel<NB, PRISM>(art, s, q, qd, imu_body, pmask);
             float* o = imu_input + (size_t)env * 9;
             o[0] = 0.0f; o[1] = 0.0f; o[2] = 0.0f; o[3] = 0.0f; o[4] = 0.0f; o[5] = 0.0f;
             o[6] = wb.x; o[7] = wb.y; o[8] = wb.z;
@@ -515,13 +539,33 @@ AGX_DEV void art_env_step(const AgxHp1Config& cfg, const AgxHp1Buffers& buf, con
 // rows double as the scratch of the sweep (parent before child): while it runs, row i >= 1 holds (P_i relative to the base origin,
 // quaternion of R_i, linear part of V_i = the velocity of the body point at the base origin, w_i), and R_l is rebuilt from row l's
 // quaternion.  A last pass turns each row into world position x_0 + P_i and origin velocity V_lin + w_i x P_i.
-template <int NB>
-AGX_DEV void art_body_states(const AgxArticulation& art, const float* root, const float* dof, float* rows) {
+// PRISM: the joint of every body i set in pmask is prismatic: R_i = R_l joint_R_i, P_i = P_l + R_l joint_p_i + a q, S_i = (0, a).
+template <int NB, bool PRISM = false>
+AGX_DEV void art_body_states(const AgxArticulation& art, const float* root, const float* dof, float* rows, uint32_t pmask = 0) {
     const int B = art.num_bodies;
 #pragma unroll
     for (int k = 0; k < 13; ++k) rows[k] = root[k];
     for (int i = 1; i < NB; ++i) {
         if (i >= B) break;
+        if constexpr (PRISM) {
+            if ((pmask >> i) & 1u) {
+                const int l = art.parent[i];
+                const float* pl = rows + 13 * l;
+                const M33 Rl = quat_to_matrix(Q4{pl[3], pl[4], pl[5], pl[6]});
+                const V3 Pl = (l == 0) ? V3{0.0f, 0.0f, 0.0f} : ld3(pl);
+                const M33 Ri = mul33(Rl, ld33(art.joint_R[i]));
+                const V3 aw = mul33v(Ri, ld3(art.axis[i]));
+                const float qi = dof[2 * (i - 1)], qd = dof[2 * (i - 1) + 1];
+                const V3 Pi = Pl + mul33v(Rl, ld3(art.joint_p[i])) + aw * qi;
+                const Q4 o = matrix_cols_to_quat(V3{Ri.m[0], Ri.m[3], Ri.m[6]}, V3{Ri.m[1], Ri.m[4], Ri.m[7]}, V3{Ri.m[2], Ri.m[5], Ri.m[8]});
+                float* r = rows + 13 * i;
+                r[0] = Pi.x; r[1] = Pi.y; r[2] = Pi.z;
+                r[3] = o.x; r[4] = o.y; r[5] = o.z; r[6] = o.w;
+                r[7] = pl[7] + aw.x * qd; r[8] = pl[8] + aw.y * qd; r[9] = pl[9] + aw.z * qd;
+                r[10] = pl[10]; r[11] = pl[11]; r[12] = pl[12];
+                continue;
+            }
+        }
         // the joint rotation first, while little else is live: sincosf's rarely taken wide-argument reduction then keeps its
         // six-word table in registers instead of a stack frame
         const V3 ax = ld3(art.axis[i]);

@@ -135,11 +135,12 @@ class ArticulationSpec:
     The MultirotorSpec beside it keeps the zero-configuration mass and inertia, which is what the controller uses.
     drive_mode: per DOF (a scalar applies to all) "position" -- the implicit drive towards the setpoints -- or "effort" -- no drive
     (its stiffness and damping are set to 0 here; the URDF <dynamics damping> stays), the engine's dof_actuation_force instead,
-    clamped to +-effort_limit where that is > 0.  effort_limit: [D] N m, default the URDF's <limit effort>."""
+    clamped to +-effort_limit where that is > 0.  effort_limit: [D] N m, default the URDF's <limit effort>.
+    The units are per DOF: a prismatic DOF (bodies.joint_kinds) has q in m, k in N / m, d in N s / m, effort and effort_limit in N."""
 
     bodies: object                     # urdf.ArticulatedBodies
-    stiffness: np.ndarray              # [D] k, N m / rad
-    damping: np.ndarray                # [D] d, N m s / rad (the URDF <dynamics damping> is added on top)
+    stiffness: np.ndarray              # [D] k, N m / rad (N / m for a prismatic DOF)
+    damping: np.ndarray                # [D] d, N m s / rad or N s / m (the URDF <dynamics damping> is added on top)
     motor_body: np.ndarray             # [M] body of each motor's application_mask link
     motor_R: np.ndarray                # [M,3,3] motor link frame in its body's frame
     motor_p: np.ndarray                # [M,3]
@@ -172,7 +173,8 @@ class ArticulationSpec:
         self.motor_body = np.asarray(self.motor_body, np.int64)
         self.motor_R, self.motor_p = np.asarray(self.motor_R, np.float64), np.asarray(self.motor_p, np.float64)
         self.motor_torque = np.asarray(self.motor_torque, np.float64)
-        # a movable subtree without inertia about its axis and without a drive would make the joint's pivot D_i zero
+        # a movable subtree without inertia about its axis (a slider's: without mass) and without a drive would make the joint's pivot
+        # D_i zero
         d_tot = self.damping + b.urdf_damping[1:]
         R0, P0 = [np.eye(3)], [np.zeros(3)]
         for i in range(1, b.num_bodies):
@@ -183,6 +185,7 @@ class ArticulationSpec:
             if self.stiffness[i - 1] > 0 or d_tot[i - 1] > 0:
                 continue
             a = R0[i] @ b.axis[i]
+            slide = b.joint_kinds[i] == "prismatic"
             J = 0.0
             for k in range(i, b.num_bodies):
                 anc = k
@@ -190,18 +193,26 @@ class ArticulationSpec:
                     anc = b.parent[anc]
                 if anc != i:
                     continue
+                if slide:  # S = (0, a): S^T I S is the subtree's mass
+                    J += float(b.mass[k])
+                    continue
                 r = P0[k] + R0[k] @ b.com[k] - P0[i]
                 Ic = R0[k] @ b.inertia[k] @ R0[k].T + b.mass[k] * (float(r @ r) * np.eye(3) - np.outer(r, r))
                 J += float(a @ Ic @ a)
             if not J > 1e-12:
                 why = "it is in effort mode and has no URDF <dynamics damping>" if self.effort_dof[i - 1] else \
                     "stiffness = damping = 0"
-                raise ValueError(f"joint '{b.joint_names[i]}': its subtree has no inertia about the axis and the joint has no drive "
+                what = "no mass to slide" if slide else "no inertia about the axis"
+                raise ValueError(f"joint '{b.joint_names[i]}': its subtree has {what} and the joint has no drive "
                                  f"({why}), so its acceleration is undefined")
 
     @property
     def num_dofs(self) -> int:
         return self.bodies.num_dofs
+
+    def prismatic_mask(self) -> int:
+        """the joint kinds for agx_hp1_articulated_step_prismatic: bit i set = body i's joint is prismatic (0: no prismatic joint)"""
+        return sum(1 << i for i, k in enumerate(self.bodies.joint_kinds) if k == "prismatic")
 
     def effort_struct(self) -> "_lib.AgxJointEffort":
         """the AgxJointEffort of the effort DOFs (its `effort` pointer left NULL)"""
@@ -324,7 +335,10 @@ class Hp1Engine:
         joint_force: with an articulation, the engine also owns joint_wrench [N,B,6] and dof_force [N,D], zero until the first step;
         physics_step then runs agx_hp1_articulated_step_joint_force (with the IMU input and the effort DOFs above, if any), which
         writes them from the last sub-step: row i >= 1 of joint_wrench is the force and the torque (about the joint origin) body i's
-        parent exerts on it through joint i, both in body i's frame, row 0 is zero; dof_force is each joint's torque along its axis."""
+        parent exerts on it through joint i, both in body i's frame, row 0 is zero; dof_force is each joint's torque along its axis.
+        An articulation with a prismatic joint runs agx_hp1_articulated_step_prismatic (with the IMU input, the effort DOFs and the
+        joint forces above, as configured) and agx_hp1_articulated_body_state_prismatic instead; its prismatic DOFs hold metres in
+        dof_state and the setpoints, N in dof_actuation_force and dof_force (the force along the slide)."""
         self.lib = _lib.load()
         self.device = torch.device(device)
         if self.device.type != "cuda":
@@ -405,9 +419,14 @@ class Hp1Engine:
     def _art_step_args(self):
         """(name, arguments but the stream) of the articulated step entry physics_step runs for this robot, from the engine's state
         at the call: with joint_force, the joint-force step (with the IMU input and the effort DOFs, if any); else with an effort
-        table, the effort step (with the IMU input, if any); else with imu_body, the IMU step; else the plain step"""
+        table, the effort step (with the IMU input, if any); else with imu_body, the IMU step; else the plain step.  A robot with a
+        prismatic joint takes the prismatic step, with whichever of these it has"""
         head = (self._cfg_ref, self._buf_ref, self._art_ref)
         imu = (self.imu_body, self.imu_input.data_ptr()) if self.imu_input is not None else (0, None)
+        if self._prismatic:  # a robot with a prismatic joint: one entry for every combination of the above
+            effort = self._effort_ref if self._effort is not None else None
+            out = (self.joint_wrench.data_ptr(), self.dof_force.data_ptr()) if self.joint_wrench is not None else (None, None)
+            return "agx_hp1_articulated_step_prismatic", head + (self._prismatic, effort) + imu + out
         if self.joint_wrench is not None:
             effort = self._effort_ref if self._effort is not None else None
             out = (self.joint_wrench.data_ptr(), self.dof_force.data_ptr())
@@ -419,10 +438,11 @@ class Hp1Engine:
         return "agx_hp1_articulated_step", head
 
     def _init_articulation(self, articulation, num_envs, debug_wrench, host_io):
-        self.articulation, self.art = articulation, None
+        self.articulation, self.art, self._prismatic = articulation, None, 0
         self.dof_state = self.dof_position_setpoint = self.dof_velocity_setpoint = None
         if articulation is None:
             return
+        self._prismatic = articulation.prismatic_mask()
         if debug_wrench:
             raise ValueError("an articulated robot has no single body wrench to report (debug_wrench)")
         if host_io:
@@ -621,6 +641,11 @@ class Hp1Engine:
         angular velocity; row 0 is root_state's.  One launch, no RNG, capturable."""
         if self.art is None:
             raise ValueError("body_state belongs to an articulated robot (Hp1Engine(articulation=...))")
+        if self._prismatic:
+            _lib.check(self.lib.agx_hp1_articulated_body_state_prismatic(
+                self._art_ref, self._prismatic, self.N, self.root_state.data_ptr(), self.root_state.stride(0), self.body_state.data_ptr(),
+                self._stream()), "agx_hp1_articulated_body_state_prismatic")
+            return
         _lib.check(self.lib.agx_hp1_articulated_body_state(self._art_ref, self.N, self.root_state.data_ptr(), self.root_state.stride(0),
                                                            self.body_state.data_ptr(), self._stream()), "agx_hp1_articulated_body_state")
 

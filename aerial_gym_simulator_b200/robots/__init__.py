@@ -103,12 +103,14 @@ class BaseROV(BaseMultirotor):
 
 
 class ArticulatedMultirotor(BaseMultirotor):
-    """A multirotor whose URDF tree has revolute / continuous joints (DESIGN.md "Articulated robots").  The controller, allocation and
+    """A multirotor whose URDF tree has revolute / continuous / prismatic joints (DESIGN.md "Articulated robots").  The controller, allocation and
     motor model are BaseMultirotor's, with the zero-configuration mass and inertia; the motors push on the bodies their links were
     merged into, and the joints are driven towards the engine's dof_position_setpoint / dof_velocity_setpoint by the drive of the
     config's joint_config (stiffness, damping per DOF; a scalar applies to every DOF).  joint_config.drive_mode ("position", the
     default, or "effort", per DOF or one for all) hands a DOF to the engine's dof_actuation_force instead, clamped to the URDF's
-    <limit effort>."""
+    <limit effort>.  Every DOF is in its joint's units: a revolute / continuous DOF in rad (k in N m / rad, d in N m s / rad, an
+    effort in N m), a prismatic DOF in m (k in N / m, d in N s / m, an effort in N) -- in dof_state_tensor, the setpoints,
+    dof_actuation_force_tensor and dof_force_tensor alike; a mixed robot gives its joint_config values as per-DOF lists."""
     articulated = True
 
     def __init__(self, robot_config, controller_name, env_config, device):
@@ -153,6 +155,7 @@ robot_registry.register("base_quadrotor_with_gimbal_camera", ArticulatedMultirot
 robot_registry.register("base_quadrotor_with_gimbal_camera_imu", ArticulatedMultirotor, rc.BaseQuadWithGimbalCameraImuCfg)
 robot_registry.register("morphy_compliant_imu", ArticulatedMultirotor, rc.MorphyCompliantImuCfg)
 robot_registry.register("base_quadrotor_with_torque_gimbal", ArticulatedMultirotor, rc.BaseQuadWithTorqueGimbalCfg)
+robot_registry.register("base_quadrotor_with_sliding_payload", ArticulatedMultirotor, rc.BaseQuadWithSlidingPayloadCfg)
 
 # the reference's package also exports its robot config classes (robots/__init__.py: `from ...base_quad_config import *`, ...)
 globals().update({_k: _v for _k, _v in vars(rc).items() if _k.endswith("Cfg")})

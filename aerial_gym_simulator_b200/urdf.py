@@ -61,20 +61,20 @@ class Joint:
     p: np.ndarray
     kind: str = "fixed"
     axis: np.ndarray = field(default_factory=lambda: np.array([1.0, 0.0, 0.0]))  # <axis xyz>, joint frame, as written
-    lower: float = 0.0  # <limit lower upper>
+    lower: float = 0.0  # <limit lower upper>: rad, m for a prismatic joint
     upper: float = 0.0
-    damping: float = 0.0  # <dynamics damping>
-    effort: float = 0.0  # <limit effort>, N m (0: none given)
+    damping: float = 0.0  # <dynamics damping>: N m s / rad, N s / m for a prismatic joint
+    effort: float = 0.0  # <limit effort>: N m, N for a prismatic joint (0: none given)
 
 
-MOVABLE_JOINTS = ("revolute", "continuous")
+MOVABLE_JOINTS = ("revolute", "continuous", "prismatic")
 
 
 @dataclass
 class ArticulatedBodies:
     """The links of a URDF merged across its fixed joints into rigid bodies (UrdfModel.articulation).  Body 0 is the root link's; body
-    i >= 1 hangs on one movable joint (DOF i - 1) and its frame is the frame of that joint's child link.  Bodies are numbered in
-    body_order()'s depth-first order, so every parent precedes its children."""
+    i >= 1 hangs on one movable joint (DOF i - 1) -- revolute, continuous or prismatic (joint_kinds) -- and its frame is the frame of
+    that joint's child link.  Bodies are numbered in body_order()'s depth-first order, so every parent precedes its children."""
     links: List[str]             # the link each body's frame is, [B]
     parent: np.ndarray           # [B] int, parent body (-1 for body 0)
     joint_names: List[str]       # [B] ("" for body 0)
@@ -84,14 +84,14 @@ class ArticulatedBodies:
     axis: np.ndarray             # [B,3] unit, body frame
     lower: np.ndarray            # [B]
     upper: np.ndarray
-    limited: np.ndarray          # [B] bool: revolute with lower < upper
+    limited: np.ndarray          # [B] bool: revolute or prismatic with lower < upper (always, for prismatic)
     urdf_damping: np.ndarray     # [B] <dynamics damping>
     mass: np.ndarray             # [B]
     com: np.ndarray              # [B,3] body frame
     inertia: np.ndarray          # [B,3,3] about the COM, body axes
     link_body: Dict[str, int]    # body each link was merged into
     link_in_body: Dict[str, Tuple[np.ndarray, np.ndarray]]  # (R, p) of each link in its body's frame
-    effort_limit: Optional[np.ndarray] = None  # [B] <limit effort>, N m (0: none; body 0: 0); None = zeros
+    effort_limit: Optional[np.ndarray] = None  # [B] <limit effort>, N m or N (0: none; body 0: 0); None = zeros
 
     def __post_init__(self):
         if self.effort_limit is None:
@@ -166,8 +166,8 @@ class UrdfModel:
 
     def articulation(self, max_bodies: int = 16) -> ArticulatedBodies:
         """The merged body table of an articulated robot.  Each body's mass, COM and inertia are the parallel-axis accumulation of
-        composite_inertia() over the links merged into it.  Joints other than fixed / revolute / continuous, a zero <axis> and more
-        than `max_bodies` bodies raise ValueError."""
+        composite_inertia() over the links merged into it.  Joints other than fixed / revolute / continuous / prismatic, a prismatic
+        joint without a <limit> with lower < upper, a zero <axis> and more than `max_bodies` bodies raise ValueError."""
         by_child = {j.child: j for j in self.joints}
         names, parent, jn, jk, jR, jp, ax, lo, hi, lim, dmp, eff = [], [], [], [], [], [], [], [], [], [], [], []
         link_body, link_in_body = {}, {}
@@ -186,7 +186,10 @@ class UrdfModel:
                 link_body[name], link_in_body[name] = b, T
                 continue
             if j.kind not in MOVABLE_JOINTS:
-                raise ValueError(f"joint '{j.name}' is {j.kind}: articulated robots support revolute and continuous joints only")
+                raise ValueError(f"joint '{j.name}' is {j.kind}: articulated robots support revolute, continuous and prismatic joints only")
+            if j.kind == "prismatic" and not j.lower < j.upper:
+                raise ValueError(f"joint '{j.name}' is prismatic without a <limit> with lower < upper ({j.lower}, {j.upper}): a slide "
+                                 "must be bounded")
             a = np.asarray(j.axis, dtype=np.float64)
             n = float(np.linalg.norm(a))
             if not n > 0:
@@ -195,7 +198,7 @@ class UrdfModel:
             link_body[name], link_in_body[name] = len(names), (np.eye(3), np.zeros(3))
             names.append(name); parent.append(link_body[j.parent]); jn.append(j.name); jk.append(j.kind)
             jR.append(Rp @ j.R); jp.append(pp + Rp @ j.p); ax.append(a / n)
-            limited = j.kind == "revolute" and j.lower < j.upper
+            limited = j.kind in ("revolute", "prismatic") and j.lower < j.upper
             lo.append(float(j.lower)); hi.append(float(j.upper)); lim.append(limited); dmp.append(float(j.damping))
             if not j.effort >= 0:
                 raise ValueError(f"joint '{j.name}' has a negative <limit effort> ({j.effort})")

@@ -235,7 +235,8 @@ int agx_hp1_check(const AgxHp1Buffers* buf, void* stream);
 
 /* ---- articulated multirotors (DESIGN.md "Articulated robots") ------------------------------------------------------------
  * A URDF tree merged across its fixed joints into rigid bodies, numbered parent before child; body 0 is the floating base (the
- * root link's body, whose row in root_state keeps its meaning), body i >= 1 hangs on one revolute / continuous joint, DOF i - 1.
+ * root link's body, whose row in root_state keeps its meaning), body i >= 1 hangs on one revolute / continuous joint, DOF i - 1 (or
+ * a prismatic one: agx_hp1_articulated_step_prismatic below).
  * Body frame = the frame of the link the body's joint points at (the root link for body 0).  Shared by all envs except the three
  * [N,...] device arrays. */
 #define AGX_ART_MAX_BODIES 16
@@ -328,6 +329,27 @@ int agx_hp1_articulated_step_joint_force(const AgxHp1Config* cfg, const AgxHp1Bu
  * allocation, no synchronisation. */
 int agx_hp1_articulated_body_state(const AgxArticulation* art, int num_envs, const float* root_state, int root_state_stride,
                                    float* body_state, void* stream);
+
+/* Prismatic joints.  prismatic_mask: bit i set = body i's joint is prismatic, a translation of body i along its unit axis by q [m]
+ * (R_i = R_parent joint_R_i, P_i = P_parent + R_parent joint_p_i + a q with a = R_i axis_i; motion subspace S_i = (0, a)); a clear
+ * bit keeps the revolute joint above.  Bit 0 must be clear, no bit may be set at or above num_bodies, and every prismatic body must
+ * be limited with lower < upper: the slide is projected onto [lower, upper] as a revolute limit is.  For a prismatic DOF the drive
+ * and effort laws are the same with q in m: k in N / m, d in N s / m, the effort and effort_limit in N; its dof_force is
+ * axis_i . (row i's force), the force along the slide, and row i's torque is about the joint origin, which moves with q. */
+
+/* agx_hp1_articulated_step_joint_force with the joint kinds of prismatic_mask, except that joint_wrench and dof_force may both be
+ * NULL (no joint forces are written and the launch uses no shared memory); where given, both 16-byte aligned (dof_force may be NULL
+ * for a one-body tree).  effort and imu_input as there (NULL: none).  A separate kernel; a robot without a prismatic joint stepped
+ * through it gets the other articulated steps' state up to float32 rounding.  Capturable: no allocation, no synchronisation. */
+int agx_hp1_articulated_step_prismatic(const AgxHp1Config* cfg, const AgxHp1Buffers* buf, const AgxArticulation* art,
+                                       uint32_t prismatic_mask, const AgxJointEffort* effort, int imu_body, float* imu_input,
+                                       float* joint_wrench, float* dof_force, void* stream);
+
+/* agx_hp1_articulated_body_state with the joint kinds of prismatic_mask (checked as in agx_hp1_articulated_step_prismatic): a
+ * prismatic body's row has the rotation of its parent's joint frame, its origin moved by a q and its velocity by a q-dot.
+ * Capturable: no RNG, no allocation, no synchronisation. */
+int agx_hp1_articulated_body_state_prismatic(const AgxArticulation* art, uint32_t prismatic_mask, int num_envs, const float* root_state,
+                                             int root_state_stride, float* body_state, void* stream);
 
 /* Masked re-initialisation, EnvManager.reset_idx for a robot-only scene
  * (env_manager/env_manager.py:273-301 -> IGE_env_manager.py:513-519, base_multirotor.py:177-205,
